@@ -1,10 +1,10 @@
-# Builds liba1mpc.so (product, sm_100a only) and the CPU oracle (test infrastructure).
+# Builds liba1mpc.so (product, sm_90a only: H100) and the CPU oracle (test infrastructure).
 NVCC ?= /usr/local/cuda/bin/nvcc
 CXX ?= g++
 PKG := a1-qp-mpc-controller_b200
 SRC := $(PKG)/csrc
 OBJ ?= build
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 EXTRA ?=
 NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xptxas -v --expt-relaxed-constexpr $(EXTRA)
 LIB ?= $(PKG)/liba1mpc.so

@@ -1,7 +1,7 @@
 """ctypes binding of liba1mpc.so (the C ABI in include/a1mpc.h).
 
 This file is glue for tests/ and bench.py: it marshals numpy arrays to the C entry points and nothing
-else.  There is no Python compute path and no fallback: if the shared library is missing or no B200 is
+else.  There is no Python compute path and no fallback: if the shared library is missing or no H100 is
 visible, construction fails loudly.  C++ hosts use include/a1mpc.h (or the ConvexMpcBatch /
 A1RobotControlBatch shims under host/) directly.
 """
@@ -205,7 +205,7 @@ class DeviceBatch:
 
 
 class Engine:
-    """one handle = one B200 + one stream (a1mpc_create / a1mpc_destroy)"""
+    """one handle = one H100 + one stream (a1mpc_create / a1mpc_destroy)"""
 
     def __init__(self, cfg=None, device=0):
         self.cfg = cfg if cfg is not None else default_config()

@@ -1,4 +1,4 @@
-// a1mpc_api.cu -- C ABI of the engine (include/a1mpc.h) over the sm_100a kernels.
+// a1mpc_api.cu -- C ABI of the engine (include/a1mpc.h) over the sm_90a kernels.
 // No CPU fallback anywhere in this file: every compute entry point launches CUDA kernels or fails.
 #include <cstdio>
 #include <cstdlib>
@@ -37,6 +37,7 @@ extern "C" void a1mpc_internal_gather_end(a1mpc_handle* h);
 struct a1mpc_handle {
   int device = 0;
   int sm_count = 0;
+  size_t l2_bytes = 0;
   cudaStream_t stream = nullptr;
   cudaStream_t side[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -274,10 +275,12 @@ int a1mpc_create(a1mpc_handle** out, const a1mpc_config* cfg, int device) {
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) return fail(A1MPC_ENODEVICE, std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) + "; this library is built for sm_100a only");
+  // architecture-specific sm_90a code loads on compute capability 9.0 and nothing else
+  if (prop.major != 9 || prop.minor != 0) return fail(A1MPC_ENODEVICE, std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) + "; this library is built for sm_90a (H100) only");
   a1mpc_handle* h = new a1mpc_handle();
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
+  h->l2_bytes = (size_t)prop.l2CacheSize;
   h->cfg = *cfg;
   DevParams& P = h->P;
   P.N = cfg->horizon;
@@ -305,8 +308,8 @@ int a1mpc_create(a1mpc_handle** out, const a1mpc_config* cfg, int device) {
     if (e != cudaSuccess) return bail(fail(A1MPC_ECUDA, std::string("kernel setup: ") + cudaGetErrorString(e)));
     e = ext_setup(cfg->horizon, h->sm_count, h->cls_ext);
     if (e != cudaSuccess) return bail(fail(A1MPC_ECUDA, std::string("ext kernel setup: ") + cudaGetErrorString(e)));
-    {   // schedules with two stance feet in every step run on the compact direct kernel (a1mpc_sched.cuh): 2.5 M instead of 1.5 M
-        // QPs/s end to end on a B200 at B = 16384 (profiles/r02a_call1_*.txt).  A1MPC_EXT_COMPACT=0 keeps everything on the general kernel (A/B).
+    {   // schedules with two stance feet in every step run on the compact direct kernel (a1mpc_sched.cuh): a problem the size of
+        // the trot problem instead of the general 4-foot one.  A1MPC_EXT_COMPACT=0 keeps everything on the general kernel (A/B).
       const char* ev = std::getenv("A1MPC_EXT_COMPACT");
       if (!(ev && ev[0] == '0') && cfg->horizon == 10) {
         e = sched2_setup(h->sm_count, h->cls_sched2);
@@ -1044,7 +1047,7 @@ int a1mpc_flush_l2(a1mpc_handle* h) {
   if (!h) return fail(A1MPC_EINVAL, "null argument");
   CK(cudaSetDevice(h->device));
   if (!h->d_flush) {
-    h->flush_elems = (size_t)256 * 1024 * 1024 / 8;  // 256 MiB > 126 MB L2
+    h->flush_elems = 2 * h->l2_bytes / 8;  // twice the L2 (50 MB on an H100): every line of it is evicted
     if (cudaMalloc(&h->d_flush, h->flush_elems * 8) != cudaSuccess) { cudaGetLastError(); return fail(A1MPC_ENOMEM, "cudaMalloc failed"); }
   }
   flush_kernel<<<h->sm_count * 8, 256, 0, h->stream>>>(h->d_flush, h->flush_elems, 1.0);
@@ -1108,15 +1111,13 @@ int a1mpc_peer_gather_wait(a1mpc_handle* h) {
   CK(cudaSetDevice(h->device));
   int* err = (int*)((char*)pg.local + (size_t)pg.nranks * 12 * pg.B * 8 + (size_t)MAX_PEERS * 8);
   // like the NCCL collect, the wait runs on the collect stream, forked after everything enqueued so far (this rank's signal included):
-  // the next solve is not held back by a slower peer; a1mpc_sync / a1mpc_event_record join it.  (Measured with the wait on the
-  // compute stream, 2 x B200, B = 1024: 0.456 ms per step against 0.414 without any collect -- every step then ends in lock-step with
-  // the slowest rank; profiles/r02_notes.md.)
+  // the next solve is not held back by a slower peer; a1mpc_sync / a1mpc_event_record join it.  (With the wait on the compute stream
+  // every step ends in lock-step with the slowest rank.)
   cudaStream_t gs = (cudaStream_t)a1mpc_internal_gather_begin(h);
   if (!gs) return fail(A1MPC_ECUDA, "could not create the collect stream");
   // Preferred: stream memory operations (cuStreamWaitValue64, >=): the wait is done by the GPU's front end and occupies no SM.  A
   // spinning wait KERNEL sits on one SM for most of every step once the compute stream runs ahead, and since the persistent solve
-  // kernels split their queue statically, one perturbed SM stretches the whole launch: measured +0.67 ms per 6.1 ms step at
-  // 2 x 32768 QPs (profiles/r02_notes.md).  The kernel (polling every 5 us, ~2 s cap) remains as the fallback.
+  // kernels split their queue statically, one perturbed SM stretches the whole launch.  The kernel (polling every 5 us, ~2 s cap) remains as the fallback.
   typedef int (*wait_value_fn)(cudaStream_t, unsigned long long, unsigned long long, unsigned int);
   static wait_value_fn wait_value = nullptr;
   static bool looked_up = false;

@@ -144,9 +144,9 @@ __global__ void __launch_bounds__(32 * WPC) solve_kernel_sched2(const __grid_con
   __syncthreads();
   const int nq = count[6];
   // QP q -> warp q % WPC of CTA q / WPC: a class with few QPs fills few CTAs completely and leaves the other SMs to the classes that
-  // run concurrently on their own streams.  (Spreading one QP per CTA first was measured in round 2: a 4-stance CTA reserves its
-  // four warps' shared memory and registers whether or not they have work, the trot class lost 2/3 of the SMs to 102 QPs and took
-  // 0.43 instead of 0.25 ms at B = 1024, while the 4-stance kernel itself did not get faster -- its time is the slowest QP's
+  // run concurrently on their own streams.  (Spreading one QP per CTA first was tried: a 4-stance CTA reserves its four warps'
+  // shared memory and registers whether or not they have work, the trot class lost most of the SMs to the 102 four-stance QPs of
+  // the benchmark batch and took far longer, while the 4-stance kernel itself did not get faster -- its time is the slowest QP's
   // factorisation count times a per-factorisation latency that one warp per scheduler already has to itself.)
   const int gw = blockIdx.x * WPC + wib, nw = gridDim.x * WPC;
   int* const head = const_cast<int*>(count) + 8 + 6;   // queue counter of this class (next_qp)

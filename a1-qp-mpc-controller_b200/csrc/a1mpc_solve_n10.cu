@@ -77,8 +77,8 @@ void fused_launch_n10(int ns, const ClassLaunch& c, cudaStream_t st, int B, cons
 #define A1MPC_N20_WPC1 2
 #endif
 #ifndef A1MPC_N20_WPC2
-#define A1MPC_N20_WPC2 3   // one CTA of three warps with the rendezvous instead of three independent one-warp CTAs: trot N = 20 B = 16384
-#endif                     // 0.55 -> 0.79 M QPs/s on a B200 (profiles/r02b_*.txt): one instruction-cache fill serves the three warps
+#define A1MPC_N20_WPC2 3   // one CTA of three warps with the rendezvous instead of three independent one-warp CTAs:
+#endif                     // one instruction-cache fill serves the three warps
 #ifndef A1MPC_N20_WPC34
 #define A1MPC_N20_WPC34 2  // wrench classes at N = 20: 106.5 KB per warp since B_k is no longer stored -> two warps per SM instead of one
 #endif

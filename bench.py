@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- convex-MPC QPs/s of the B200 engine (and, with --impl reference, of the CPU restatement
+"""bench.py -- convex-MPC QPs/s of the H100 engine (and, with --impl reference, of the CPU restatement
 of the reference path).  One JSON line on stdout (rank 0).
 
 A "step" is one a1mpc_solve_batch over one batch of synthetic trot-gait states:
@@ -10,6 +10,9 @@ Weak scaling: every rank solves its own B QPs (independent slices, no data-path 
 
 Timing: CUDA events on the handle's stream around exactly K steps after W warm-up steps, barrier + device
 synchronise on both sides, max over ranks.  Inputs rotate through a ring of distinct batches larger than L2.
+
+--dump-outputs DIR: after the timed steps, the arrays the last timed step handed its caller (f_body [12][B] and status [B], as
+float64 .npy files) go to DIR, so that two builds can be compared output for output; the inputs depend only on the arguments.
 """
 import argparse
 import json
@@ -27,7 +30,7 @@ sys.path.insert(0, ROOT)
 
 METRIC = "convex-MPC QPs/sec (N=10, batched)"
 UNIT = "QPs/s"
-L2_BYTES = 126e6
+L2_BYTES = 50 * 2 ** 20            # H100 SXM: 50 MB of L2
 IN_BYTES_PER_QP = 42 * 8 + 4     # x0[12] rot[9] foot[12] ref[9] fp64 + contact mask
 OUT_BYTES_PER_QP = 12 * 8 + 4    # f_body[12] fp64 + status
 ALG_BYTES_PER_QP = IN_BYTES_PER_QP + OUT_BYTES_PER_QP   # 440 B (SURVEY 8d)
@@ -60,7 +63,7 @@ def algorithmic_flops(N, ns_hist, fact_by_class):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons while the GPU is under load (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks/throttle reasons while the GPU is under load"""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -259,7 +262,7 @@ def _status_hist(a1mpc, eng, d, B):
 
 def subrecord_config3(a1mpc, local, K=20, W=3):
     """BASELINE configs[2]: trot, N = 20, batch 8192, precision 32 (fp32 boundary arrays, fp64 + certificate inside), 1 GPU.
-    4 distinct device-resident batches, L2 flushed before every step (the flush, ~40 us, is inside the timed region: < 0.3 %)."""
+    4 distinct device-resident batches, L2 flushed before every step (the flush is inside the timed region)."""
     B, N = 8192, 20
     eng = a1mpc.Engine(a1mpc.default_config(horizon=N, precision=32), device=local)
     dev = []
@@ -345,7 +348,7 @@ def subrecord_config5(a1mpc, eng, dist, n_gpus, rank, collect_mode, K=30, W=3):
            "value": n_gpus * B / (ms * 1e-3), "unit": UNIT, "ms_per_step": ms, "steps": K, "warmup": W, "dtype": "f64", "n_gpus": n_gpus,
            "final_collect": desc if fn is not None else ("none" if not collect_mode else "unavailable: %s" % err), "peer_wait_timeouts": peer_status, "final_collect_verified": verified,
            "status_histogram_rank0": _status_hist(a1mpc, eng, dev[0], B),
-           "cache": "4 distinct batches per rank (4 x 11 MB in, outputs 3 MB): smaller than L2, the path is compute bound (440 B against ~1 MFLOP per QP)"}
+           "cache": "4 distinct batches per rank (4 x 11 MB in, 4 x 3 MB out: about the 50 MB of L2), the path is compute bound (440 B against ~1 MFLOP per QP)"}
     for d in dev:
         d.free()
     return rec
@@ -393,6 +396,22 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
+DUMP_MAX_BYTES = 64 * 2 ** 20
+
+
+def dump_outputs(out_dir, f_body, status):
+    """f_body [12][B] and status [B] as float64; above DUMP_MAX_BYTES a fixed seeded sample of QPs (indices in qp_index.npy)"""
+    os.makedirs(out_dir, exist_ok=True)
+    B = status.shape[0]
+    per_qp = 8 * (f_body.shape[0] + 2)
+    if B * per_qp > DUMP_MAX_BYTES:
+        idx = np.sort(np.random.default_rng(0).choice(B, DUMP_MAX_BYTES // per_qp, replace=False))
+        f_body, status = f_body[:, idx], status[idx]
+        np.save(os.path.join(out_dir, "qp_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "f_body.npy"), np.ascontiguousarray(f_body, dtype=np.float64))
+    np.save(os.path.join(out_dir, "status.npy"), status.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -408,6 +427,7 @@ def main():
     ap.add_argument("--collect", default="auto", choices=["auto", "peer", "nccl"], help="final collect for --gpus > 1")
     ap.add_argument("--ring", type=int, default=0, help="number of distinct input batches (0: enough to exceed L2)")
     ap.add_argument("--no-subrecords", action="store_true", help="skip the config3 / config4 / config5 sub-records")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -477,6 +497,8 @@ def main():
     t_wall1 = time.time()
     ms_local = eng.elapsed_ms(e0, e1)
     class_ms, ncalls = eng.profile_end()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *dev[(W + K - 1) % ring].download())
     launches = eng.launches() - launches0
     ms = dist_max(dist, ms_local)
     value = n_gpus * B * K / (ms * 1e-3)
@@ -555,13 +577,8 @@ def main():
     hist = {ns: int((ns_of == ns).sum()) for ns in range(5)}
     dom = int(np.argmax(class_ms)) + 1
     dom_ms = class_ms[dom - 1] / max(ncalls, 1)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm_peak = 3350.0
+    peak_src = "H100 SXM data sheet (HBM3, 3.35 TB/s at up to 700 W); assumes the SXM part: an H100 PCIe or NVL has another HBM peak"
     dom_qps = hist.get(dom, 0)
     achieved_gbs = ALG_BYTES_PER_QP * dom_qps / (dom_ms * 1e-3) / 1e9 if dom_ms > 0 else 0.0
     it_by_class = {}
@@ -585,7 +602,7 @@ def main():
                 "peak_source": peak_src,
                 "algorithmic_bytes_per_qp": ALG_BYTES_PER_QP, "qps_per_launch": dom_qps, "kernel_ms": dom_ms,
                 "note": "the path is fp64-pipe/latency bound (SURVEY 8d: ~1e4 FLOP/B), so the HBM fraction is small by construction; see roofline_fp64"}
-    roofline_fp64 = {"bound": "fp64 pipes (DFMA + DMMA.8x8x4; the tensor and the vector fp64 peak of a B200 are about equal)", "kernel": roofline["kernel"], "unit": "TFLOP/s",
+    roofline_fp64 = {"bound": "fp64 pipes (DFMA + DMMA.8x8x4; the peak is the measured DFMA rate, an H100's DMMA peak is about twice its DFMA peak)", "kernel": roofline["kernel"], "unit": "TFLOP/s",
                      "achieved_algorithmic": fl_alg / (dom_ms * 1e-3) / 1e12 if dom_ms > 0 else 0.0,
                      "achieved_executed": fl_exec / (dom_ms * 1e-3) / 1e12 if dom_ms > 0 else 0.0,
                      "peak": fp64_peak, "peak_source": "measured in this run (a1mpc_measure_fp64_peak: dependent-free DFMA stream)",
@@ -604,7 +621,7 @@ def main():
             "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": {"workload": "trot gait convex MPC, horizon N=%d, batch %d per GPU, fp64 (BASELINE configs[1]%s)" % (N, B, "" if (B == 1024 and N == 10) else " variant"),
                        "horizon": N, "batch_per_gpu": B, "global_batch": B * n_gpus, "generator": "a1mpc_gen_states config_id=%d" % args.config_id,
-                       "cache": "inputs rotate through a ring of %d distinct batches = %.0f MB %s L2 (126 MB)" % (ring, ring_bytes / 1e6, ">" if ring_bytes > L2_BYTES else "< (NOT larger than)"),
+                       "cache": "inputs rotate through a ring of %d distinct batches = %.0f MB %s L2 (50 MB)" % (ring, ring_bytes / 1e6, ">" if ring_bytes > L2_BYTES else "< (NOT larger than)"),
                        "stance_feet_histogram": hist,
                        "final_collect_verified": collect_ok,
                        "final_collect": (collect_desc if collect_fn is not None else ("none" if n_gpus == 1 or args.no_gather else "unavailable: %s" % collect_err))},

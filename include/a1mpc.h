@@ -1,5 +1,5 @@
 /*
- * a1mpc.h -- C ABI of the B200-native batched convex-MPC QP engine.
+ * a1mpc.h -- C ABI of the H100-native batched convex-MPC QP engine.
  *
  * Drop-in boundary for the hot path of ShuoYangRobotics/A1-QP-MPC-Controller:
  *   ConvexMpc            (src/a1_cpp/src/ConvexMpc.h:22-94,  ConvexMpc.cpp:7-260)
@@ -65,7 +65,7 @@ typedef struct a1mpc_handle a1mpc_handle;
  *                        reinterpreted.  The arithmetic in between stays fp64 with the in-kernel KKT certificate: the reduced
  *                        systems have condition numbers of 1e5 (N=10) .. 1e6 (N=20), an fp32 factorisation cannot certify
  *                        1e-4 N, and the only fp32-input tensor-core MMA (tf32, 10-bit mantissa) breaks down on 85 % of the
- *                        QPs (profiles/r01_notes.md).  Accuracy contract: the returned forces are the exact optimum of the QP
+ *                        QPs.  Accuracy contract: the returned forces are the exact optimum of the QP
  *                        posed by the fp32-rounded inputs, rounded to fp32 -- |f - f*(rounded inputs)| <= 1e-4 N + 1 fp32 ulp.
  *                        The parity / neighbouring entry points (build_qp, qp_mats, solve_dense, grf_qp, torques, plan,
  *                        kinematics, EKF) are fp64 whatever this field says.

@@ -1,6 +1,6 @@
 """The device code of a1mpc_device.cuh on the lane-accurate CPU emulator (tests/emu/) against the oracle.
 
-Test infrastructure, not a product path: the SAME kernels nvcc compiles for sm_100a are compiled by g++ against an
+Test infrastructure, not a product path: the SAME kernels nvcc compiles for sm_90a are compiled by g++ against an
 emulation of the warp primitives (shuffles, ballots, mma.m8n8k4.f64 fragments, __syncwarp) and run one fibre per CUDA
 thread.  This catches, without a GPU, what the oracle alone cannot: wrong fragment/lane maps, wrong shared-memory tile
 addressing, missing barriers (results must not depend on the order in which the lanes of a warp run between two
@@ -131,7 +131,7 @@ def test_grf_qp_on_emulator(E, a1, O):
 
 
 def test_degenerate_vertex_family_is_certified(E, a1, O):
-    """The one QP of the 1.44 M robustness sweep on the B200 (profiles/r01d_robust_sweep_dmma.txt) that ended IPM_ONLY, with
+    """The one QP of the 1.44 M robustness sweep on the GPU that ended IPM_ONLY, with
     1e-9 perturbations: at one foot-step the optimum is the cone vertex with a degenerate multiplier; release (dual violation
     4e-11, just above the 1e-11 certificate tolerance) and re-pin (fz = -2.6e-7) alternated for all 36 rounds.  Without the
     residual-driven refinement of the reduced solves (variant "nohyst": fixed step count as in round 1, no hysteresis either) the
@@ -255,7 +255,7 @@ def test_edge_cases_on_emulator(E, a1, O):
 def test_certified_means_optimal_every_qp_checked(E, a1, O):
     """OPTIMAL must mean optimal.  (1) The QPs that round 1's certificate got wrong -- stationarity on the free coordinates was
     assumed after the linear solve; three stance feet, Woodbury residual 3e-4, certified 1.8e-2 N / 5.9e-4 N off -- and the two
-    warm-started ones that the finisher hysteresis certified 2e-4 N / 1.7e-5 N off (profiles/r01_notes.md).  (2) Every QP of a
+    warm-started ones that the finisher hysteresis certified 2e-4 N / 1.7e-5 N off.  (2) Every QP of a
     batch with random stance patterns against the oracle, not a sample."""
     cfg = a1.default_config(horizon=10)
     d = dict(np.load(os.path.join(ROOT, "tools", "data", "false_certificates_r01.npz")))

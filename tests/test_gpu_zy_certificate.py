@@ -1,6 +1,6 @@
 """OPTIMAL must mean optimal -- on the GPU, through the C ABI, EVERY QP of a batch against the oracle (not a sample), plus the QPs
 that round 1's certificate got wrong (found on the CPU emulator after the round's GPU minutes were spent: stationarity on the
-free coordinates was assumed after the linear solve; profiles/r01_notes.md).  Same checks as
+free coordinates was assumed after the linear solve).  Same checks as
 tests/test_emu.py::test_certified_means_optimal_every_qp_checked."""
 import os
 

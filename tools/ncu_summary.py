@@ -1,4 +1,4 @@
-"""dev tool: text summary of an .ncu-rep (raw page) for profiles/"""
+"""dev tool: text summary of an .ncu-rep (raw page)"""
 import csv, subprocess, sys
 rep = sys.argv[1]
 raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

@@ -18,7 +18,6 @@ for N, wname, cid, B in ((10, "gazebo", 2, 524288), (10, "gazebo", 4, 524288), (
     bad = np.nonzero(status != 0)[0]
     print("N=%d %s cid=%d B=%d: %.2fs status hist %s  ipm max %d rounds max %d" % (N, wname, cid, B, dt, np.bincount(status, minlength=5), (iters % 100).max(), (iters // 100).max()), flush=True)
     # every QP against the oracle, not a sample: round 1's 1 500 spot checks missed 1-in-70 000 certified-but-wrong answers
-    # (profiles/r01_notes.md); the oracle's exact mode does ~6 000 QPs/s per 8 cores at N = 10
     nfull = B if N == 10 else min(B, 20000)
     chk = np.concatenate([bad[:20], np.arange(nfull)])
     sub = {k: (v[chk].copy() if k == "contact" else v[:, chk].copy()) for k, v in st.items()}

@@ -1,5 +1,5 @@
 #!/bin/bash
-# dev tool: SASS evidence of the tensor-core / TMA / mbarrier paths in the shipped library (profiles/r02_sass_mnemonics.txt)
+# dev tool: SASS evidence of the tensor-core / TMA / mbarrier paths in the shipped library
 LIB=${1:-a1-qp-mpc-controller_b200/liba1mpc.so}
 echo "# cuobjdump -sass $LIB  ($(date -u +%Y-%m-%d), $(nvcc --version | grep release | sed 's/.*release //'))"
 echo "# per kernel: count of DMMA.8x8x4 (fp64 tensor-core MMA), UBLKCP (cp.async.bulk TMA copy), SYNCS.* (mbarrier arrive / try_wait), DFMA"
