@@ -26,6 +26,13 @@ void ext_launch(int horizon, const ClassLaunch& c, cudaStream_t st, int B, const
 // compacted two-stance-feet-per-step class of the extended path (a1mpc_sched.cuh; opt-in, N = 10)
 cudaError_t sched2_setup(int sm_count, ClassLaunch& c);
 void sched2_launch(const ClassLaunch& c, cudaStream_t st, int B, const DevParams& P, const double* rec, const int* count, const DevOutputs& out);
+// warm-started variants of both (a1mpc_solve_batch_ext_warm, N = 10)
+cudaError_t ext_warm_setup(int sm_count, ClassLaunch& c);
+void ext_warm_launch(const ClassLaunch& c, cudaStream_t st, int B, const DevParams& P, const double* rec, const int* count, const DevOutputs& out,
+                     uint32_t* warm, int shift);
+cudaError_t sched2_warm_setup(int sm_count, ClassLaunch& c);
+void sched2_warm_launch(const ClassLaunch& c, cudaStream_t st, int B, const DevParams& P, const double* rec, const int* count, const DevOutputs& out,
+                        uint32_t* warm, int shift);
 cudaError_t build_dense_launch(const DevParams& P, const DevInputs& in, int B, double* H, double* g, double* lb, double* ub, cudaStream_t st);
 
 // QP-major side entry points (a1mpc_dense.cu)

@@ -133,6 +133,16 @@ __global__ void pack_ext2_kernel(DevInputs in, const uint32_t* __restrict__ sche
   }
 }
 
+// a1mpc_solve_batch_ext_warm: a robot without contact anywhere in its schedule never reaches a solve kernel (the pack kernels
+// answer it), so its warm-start slot is cleared here: it stores no guess, like a robot that ended NUMERICAL
+__global__ void warm_forget_no_contact_kernel(DevInputs in, const uint32_t* __restrict__ sched, int B, uint32_t* __restrict__ warm, int horizon) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  uint32_t any = 0u;
+  for (int st = 0; st < horizon; ++st) any |= (sched ? sched[(size_t)st * in.ld + b] : in.contact[b]) & 15u;
+  if (any == 0u) warm[(size_t)b * (WARM_HDR + 4 * horizon)] = 0u;
+}
+
 // Classes whose factor does not fit in shared memory (N=20 with four stance feet in fp64):
 // reported, never silently approximated.
 __global__ void unsupported_kernel(const double* __restrict__ rec, const int* __restrict__ count, int cls, DevOutputs out, int horizon) {

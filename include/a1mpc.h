@@ -161,6 +161,19 @@ typedef struct a1mpc_inputs_ext {
 } a1mpc_inputs_ext;
 int  a1mpc_solve_batch_ext(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_inputs_ext* ext, const a1mpc_outputs* out);
 
+/* ---- warm start of the scheduled call: a1mpc_solve_batch_ext + the device-resident warm start above -------------------
+ * Same contract as a1mpc_solve_batch_ext (host or device arrays, precision 32, isotropic r with normals) plus `warm` and
+ * `shift` as in a1mpc_solve_batch_warm (same buffer: a1mpc_warm_bytes / a1mpc_warm_reset).  The slot keeps the verified face of
+ * every (horizon step, leg) together with the schedule it was solved for; the guess for foot-step (st, leg) in contact now is
+ * the stored face of (st + shift, leg) (step N-1 past the end) if that foot-step was in contact then, and the free face if it
+ * was not.  A schedule produced by a1mpc_update_plan_batch moves by one step per control tick: shift = 1.  A robot whose
+ * guess does not verify takes the cold path inside the same launch; OPTIMAL is KKT-certified either way.  Slots written by
+ * a1mpc_solve_batch_warm are "no guess" here and the reverse; robots that end NUMERICAL or have no contact store no guess.
+ * ext NULL (or both fields NULL) = a1mpc_solve_batch_warm.  A1MPC_EINVAL: horizon 20, shift outside [0, N], `warm` not device
+ * memory. */
+int  a1mpc_solve_batch_ext_warm(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_inputs_ext* ext, const a1mpc_outputs* out,
+                                void* warm, int shift);
+
 /* ---- ConvexMpc members, for parity with the reference class (ConvexMpc.h:87-93) ----------- */
 /* Dense QP data exactly as ConvexMpc::calculate_qp_mats leaves it after compute_grf drove it
  * (constant B_d over the horizon, A1RobotControl.cpp:498-514).  QP-major outputs:
