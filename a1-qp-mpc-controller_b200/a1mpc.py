@@ -18,7 +18,8 @@ STATUS_OPTIMAL, STATUS_IPM_ONLY, STATUS_MAXITER, STATUS_NUMERICAL, STATUS_NO_CON
 EXPORTS = [
     "a1mpc_default_config", "a1mpc_create", "a1mpc_destroy", "a1mpc_last_error", "a1mpc_device_count",
     "a1mpc_solve_batch", "a1mpc_warm_bytes", "a1mpc_warm_reset", "a1mpc_solve_batch_warm", "a1mpc_solve_batch_ext", "a1mpc_solve_batch_ext_warm", "a1mpc_build_qp_batch", "a1mpc_qp_mats_batch", "a1mpc_solve_dense_batch",
-    "a1mpc_grf_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch", "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
+    "a1mpc_grf_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
+    "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
     "a1mpc_flush_l2", "a1mpc_profile_begin", "a1mpc_profile_end", "a1mpc_nccl_unique_id", "a1mpc_nccl_init", "a1mpc_allgather_forces",
@@ -116,6 +117,11 @@ def lib():
         l.a1mpc_grf_qp_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
         l.a1mpc_joint_torques_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
         l.a1mpc_update_plan_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams)] + [C.c_void_p] * 13
+        l.a1mpc_swing_bytes.restype = C.c_size_t
+        l.a1mpc_swing_bytes.argtypes = [C.c_int]
+        l.a1mpc_swing_init_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        l.a1mpc_swing_legs_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_double] + [C.c_void_p] * 10
+        l.a1mpc_terrain_pitch_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         l.a1mpc_gen_states.argtypes = [C.c_int, C.c_uint64, C.c_int] + [C.c_void_p] * 5
         l.a1mpc_measure_fp64_peak.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         l.a1mpc_profile_begin.argtypes = [C.c_void_p, C.c_int]
@@ -386,6 +392,42 @@ class Engine:
         _check(lib().a1mpc_memcpy_d2h(self.h, _p(buf), ekf, buf.nbytes))
         _check(lib().a1mpc_sync(self.h))
         return buf[:, :18].copy(), buf[:, 18:].reshape(B, 18, 18).copy()
+
+    def swing_alloc(self, B):
+        """device-resident swing-leg / terrain controller state of B robots (a1mpc_swing_bytes), initialised by a1mpc_swing_init_batch;
+        bound to this B"""
+        p = self.dalloc(lib().a1mpc_swing_bytes(B))
+        self.swing_init(p, B)
+        return p
+
+    def swing_init(self, swing, B):
+        """a1mpc_swing_init_batch: A1CtrlStates::reset() values and empty filters"""
+        _check(lib().a1mpc_swing_init_batch(self.h, B, swing))
+
+    def swing_legs(self, gp, kp_foot, kd_foot, swing, dt, gait_counter, plan_contacts, rot_z, foot_pos_abs, foot_pos_target_rel, foot_force):
+        """a1mpc_swing_legs_batch (generate_swing_legs_ctrl), host arrays: gait_counter [4,B], plan_contacts [B], rot_z [9,B],
+        foot_pos_abs / foot_pos_target_rel [12,B], foot_force [4,B]; kp_foot, kd_foot [12] leg-major ->
+        f_kin [12,B], contacts [B], foot_pos_cur [12,B], foot_pos_recent_contact [12,B]"""
+        kp, kd, gc = [np.ascontiguousarray(v, dtype=np.float64) for v in (kp_foot, kd_foot, gait_counter)]
+        pc = np.ascontiguousarray(plan_contacts, dtype=np.uint32)
+        a = [np.ascontiguousarray(v, dtype=np.float64) for v in (rot_z, foot_pos_abs, foot_pos_target_rel, foot_force)]
+        B = pc.shape[0]
+        fk = np.zeros((12, B)); con = np.zeros(B, dtype=np.uint32); cur = np.zeros((12, B)); rc = np.zeros((12, B))
+        _check(lib().a1mpc_swing_legs_batch(self.h, B, C.byref(gp), _p(kp), _p(kd), swing, C.c_double(dt), _p(gc), _p(pc), *[_p(v) for v in a],
+                                            _p(fk), _p(con), _p(cur), _p(rc)))
+        return fk, con, cur, rc
+
+    def terrain_pitch(self, swing, use_terrain_adapt, root_pos, ref=None):
+        """a1mpc_terrain_pitch_batch, host arrays: root_pos [3,B]; ref [9,B] (a1mpc_inputs.ref layout) gets row 1 in place when
+        use_terrain_adapt -> terrain_pitch [B]"""
+        pos = np.ascontiguousarray(root_pos, dtype=np.float64)
+        B = pos.shape[1]
+        if ref is not None and not (ref.dtype == np.float64 and ref.flags["C_CONTIGUOUS"]):
+            raise A1MpcError("ref must be a C-contiguous float64 array (written in place)")
+        pitch = np.zeros(B)
+        _check(lib().a1mpc_terrain_pitch_batch(self.h, B, swing, int(use_terrain_adapt), _p(pos), _p(ref), ref.shape[1] if ref is not None else B,
+                                               _p(pitch)))
+        return pitch
 
     def update_plan(self, gp, gait_counter, gait_counter_speed, movement_mode, lin_vel, lin_vel_d, rot_z, rot, root_pos):
         """A1RobotControl::update_plan batched; returns new gait_counter [4,B], plan_contacts [B], contact_sched [N,B],

@@ -12,6 +12,7 @@
 #include "a1mpc_internal.h"
 #include "a1mpc_misc.cuh"
 #include "a1mpc_estim.cuh"
+#include "a1mpc_swing.cuh"
 
 using namespace a1mpc;
 
@@ -935,6 +936,90 @@ int a1mpc_ekf_update_batch(a1mpc_handle* h, int B, void* ekf_state, double dt, i
   if (grid > h->sm_count * 2) grid = h->sm_count * 2;
   ekf_update_kernel<<<grid, 32 * EKF_WPC, smem, h->stream>>>(B, P, static_cast<double*>(ekf_state), movement_mode, imu_acc, imu_ang_vel, rot,
                                                              foot_pos_rel, foot_vel_rel, foot_force, root_pos, root_lin_vel, estimated_contacts, status);
+  h->launches++;
+  CK(cudaGetLastError());
+  return st.finish();
+}
+
+// ---- swing-leg control and terrain pitch (generate_swing_legs_ctrl, compute_grf's terrain adaptation) --------------------------
+size_t a1mpc_swing_bytes(int B) { return B > 0 ? (size_t)B * SW_FIELDS * sizeof(double) : 0; }
+
+int a1mpc_swing_init_batch(a1mpc_handle* h, int B, void* swing_state) {
+  if (!h || !swing_state) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
+  swing_init_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, static_cast<double*>(swing_state));
+  h->launches++;
+  CK(cudaGetLastError());
+  return A1MPC_OK;
+}
+
+int a1mpc_swing_legs_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, const double* kp_foot, const double* kd_foot, void* swing_state,
+                           double dt, const double* gait_counter, const uint32_t* plan_contacts, const double* rot_z, const double* foot_pos_abs,
+                           const double* foot_pos_target_rel, const double* foot_force, double* f_kin, uint32_t* contacts, double* foot_pos_cur,
+                           double* foot_pos_recent_contact) {
+  if (!h || !gp || !kp_foot || !kd_foot || !swing_state || !gait_counter || !plan_contacts || !rot_z || !foot_pos_abs || !foot_pos_target_rel ||
+      !foot_force || !f_kin || !contacts)
+    return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (!(dt > 0.0) || !(gp->counter_per_swing > 0.0)) return fail(A1MPC_EINVAL, "dt and counter_per_swing must be positive");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
+  if (is_device_ptr(kp_foot) || is_device_ptr(kd_foot)) return fail(A1MPC_EINVAL, "kp_foot and kd_foot are host arrays (batch-uniform parameters)");
+  const bool dev = is_device_ptr(gait_counter);
+  if (mixed_sides(dev, {plan_contacts, rot_z, foot_pos_abs, foot_pos_target_rel, foot_force, f_kin, contacts, foot_pos_cur, foot_pos_recent_contact}))
+    return fail(A1MPC_EINVAL, "batch arrays must be all-host or all-device (kp_foot, kd_foot: always host)");
+  SwingParams P;
+  P.cps = gp->counter_per_swing;
+  P.dt = dt;
+  for (int i = 0; i < 12; ++i) { P.kp[i] = kp_foot[i]; P.kd[i] = kd_foot[i]; }
+  const size_t Bs = (size_t)B;
+  Stage st{h, !dev};
+  int rc;
+  if (st.host) {
+    if ((rc = ensure_side(h, 11 * Stage::pad(12 * Bs * 8)))) return rc;
+    st.cur = (char*)h->d_side;
+  }
+  if ((rc = st.in(gait_counter, 4 * Bs * 8))) return rc;
+  if ((rc = st.in(plan_contacts, Bs * 4))) return rc;
+  if ((rc = st.in(rot_z, 9 * Bs * 8))) return rc;
+  if ((rc = st.in(foot_pos_abs, 12 * Bs * 8))) return rc;
+  if ((rc = st.in(foot_pos_target_rel, 12 * Bs * 8))) return rc;
+  if ((rc = st.in(foot_force, 4 * Bs * 8))) return rc;
+  st.out(f_kin, 12 * Bs * 8); st.out(contacts, Bs * 4); st.out(foot_pos_cur, 12 * Bs * 8); st.out(foot_pos_recent_contact, 12 * Bs * 8);
+  swing_legs_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, P, static_cast<double*>(swing_state), gait_counter, plan_contacts, rot_z, foot_pos_abs,
+                                                            foot_pos_target_rel, foot_force, f_kin, contacts, foot_pos_cur, foot_pos_recent_contact);
+  h->launches++;
+  CK(cudaGetLastError());
+  return st.finish();
+}
+
+int a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref, size_t ref_ld,
+                              double* terrain_pitch) {
+  if (!h || !swing_state || !root_pos || (use_terrain_adapt && !ref)) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (ref && ref_ld < (size_t)B) return fail(A1MPC_EINVAL, "ref_ld must be >= B");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
+  const bool dev = is_device_ptr(root_pos);
+  if (mixed_sides(dev, {ref, terrain_pitch})) return fail(A1MPC_EINVAL, "batch arrays must be all-host or all-device");
+  const size_t Bs = (size_t)B;
+  // only row 1 of ref is written: on the host side it is staged as a dense row (ld 0 from the kernel's point of view)
+  double* row = use_terrain_adapt ? ref + ref_ld : nullptr;
+  size_t kld = ref_ld;
+  Stage st{h, !dev};
+  int rc;
+  if (st.host) {
+    if ((rc = ensure_side(h, 3 * Stage::pad(3 * Bs * 8)))) return rc;
+    st.cur = (char*)h->d_side;
+    kld = 0;
+  }
+  if ((rc = st.in(root_pos, 3 * Bs * 8))) return rc;
+  st.out(row, Bs * 8); st.out(terrain_pitch, Bs * 8);
+  double* kref = st.host ? row : ref;
+  terrain_pitch_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, static_cast<double*>(swing_state), use_terrain_adapt ? 1 : 0, root_pos, kref, kld,
+                                                               terrain_pitch);
   h->launches++;
   CK(cudaGetLastError());
   return st.finish();

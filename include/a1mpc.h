@@ -278,6 +278,42 @@ int  a1mpc_update_plan_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp
                              const double* rot, const double* root_pos, uint32_t* plan_contacts, uint32_t* contact_sched,
                              double* foot_pos_target_rel, double* foot_pos_target_abs, double* foot_pos_target_world);
 
+/* ---- the stages between update_plan and the path: A1RobotControl::generate_swing_legs_ctrl and compute_grf's terrain adaptation ----
+ * generate_swing_legs_ctrl (A1RobotControl.cpp:204-287) produces the `contact` of a1mpc_solve_batch* and the f_kin / contact of
+ * a1mpc_joint_torques_batch; the front of compute_grf (:334-376, compute_walking_surface :566-582) poses root_euler_d[1] on a slope.
+ * The controller state they keep lives on the device: a1mpc_swing_bytes(B) bytes (a1mpc_device_alloc), per robot the fields
+ * foot_pos_start, foot_pos_rel_last_time, foot_pos_target_last_time, foot_pos_recent_contact, early_contacts and the thirteen
+ * moving-window filters (recent_contact_{x,y,z}_filter[4] of 60 samples, terrain_angle_filter of 100).  The layout is opaque and
+ * batch-major, so a buffer is bound to the B it was initialised for: pass the same B to every call on it.
+ *   a1mpc_swing_init_batch     A1CtrlStates::reset() values of those fields (A1CtrlStates.h:83-100) and fresh filters
+ *                              (A1RobotControl.cpp:52-57): zero positions, no early contact, empty windows
+ *   a1mpc_swing_legs_batch     one generate_swing_legs_ctrl tick: foot_pos_cur = R_z^T foot_pos_abs; stance legs (gait_counter <=
+ *                              counter_per_swing) refresh foot_pos_start, swing legs follow the degree-4 Bezier from foot_pos_start to
+ *                              foot_pos_target_rel with spline time float(gc - cps) / float(cps) and the clearances 0.0f / 0.4f of
+ *                              A1Params.h:41-42; finite-difference velocities over dt; f_kin = kp .* pos_error + kd .* vel_error;
+ *                              early contact (sticky until gc <= 1.5 cps) when a swing foot past 1.5 cps feels more than FOOT_FORCE_LOW
+ *                              = 30 N; contacts = plan | early; on contact ticks the leg's recent-contact filters take foot_pos_abs.
+ *                              gp: counter_per_swing only.  kp_foot[12], kd_foot[12] (leg-major: FL(x,y,z), FR, RL, RR): batch-uniform
+ *                              HOST arrays, like km_foot.  Batch-major SoA (ld = B), host or device: gait_counter [4][B] (after
+ *                              a1mpc_update_plan_batch), plan_contacts [B], rot_z [9][B] root_rot_mat_z, foot_pos_abs [12][B],
+ *                              foot_pos_target_rel [12][B], foot_force [4][B]; out: f_kin [12][B] (foot_forces_kin), contacts [B];
+ *                              foot_pos_cur, foot_pos_recent_contact [12][B] (may be NULL).
+ *   a1mpc_terrain_pitch_batch  least-squares plane through the four recent-contact points (pseudo-inverse with the reference's
+ *                              cutoff eps * 3 * sigma_max), dihedral angle to flat ground, averaged by the 100-sample filter only while
+ *                              root_pos z > 0.1 (0 otherwise), clipped to +-0.5; the sign is - when the front feet stand more than
+ *                              0.05 m above the rear ones.  root_pos [3][B]; ref [9][B] with leading dimension ref_ld >= B, an
+ *                              a1mpc_inputs.ref array: only row 1 (root_euler_d[1]) is written, and only when use_terrain_adapt (ref may
+ *                              be NULL otherwise); terrain_pitch [B] out (terrain_pitch_angle, may be NULL).
+ * swing_state must be device memory (A1MPC_EINVAL otherwise); the batch arrays of one call are all host or all device. */
+size_t a1mpc_swing_bytes(int B);
+int  a1mpc_swing_init_batch(a1mpc_handle* h, int B, void* swing_state);
+int  a1mpc_swing_legs_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, const double* kp_foot, const double* kd_foot, void* swing_state,
+                            double dt, const double* gait_counter, const uint32_t* plan_contacts, const double* rot_z, const double* foot_pos_abs,
+                            const double* foot_pos_target_rel, const double* foot_force, double* f_kin, uint32_t* contacts, double* foot_pos_cur,
+                            double* foot_pos_recent_contact);
+int  a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref, size_t ref_ld,
+                               double* terrain_pitch);
+
 /* ---- device memory, stream and timing helpers (so hosts need no CUDA headers) -------------- */
 int  a1mpc_device_alloc(a1mpc_handle* h, size_t bytes, void** ptr);
 int  a1mpc_device_free(a1mpc_handle* h, void* ptr);
