@@ -238,8 +238,9 @@ class Engine:
             pass
 
     # ---- hot path ----
-    def solve(self, st, want_u=False):
-        """host arrays in, host arrays out (H2D + kernels + D2H inside the call)"""
+    def _solve(self, fn, st, want_u=False, ext=None, warm_args=()):
+        """one a1mpc_solve_batch* call on host arrays: ext = (sched [N,B] or None, normals [12,B] or None) for the _ext calls,
+        warm_args = (warm, shift) for the _warm calls"""
         B = st["x0"].shape[1]
         N = self.cfg.horizon
         ft = self.ftype     # float32 arrays at the boundary when cfg.precision == 32
@@ -248,8 +249,17 @@ class Engine:
         u = np.zeros((12 * N, B), dtype=ft) if want_u else None
         inp = Inputs(_p(a["x0"]), _p(a["rot"]), _p(a["foot"]), _p(a["ref"]), _p(a["contact"]), B)
         out = Outputs(_p(f), _p(status), _p(iters), _p(u), B)
-        _check(lib().a1mpc_solve_batch(self.h, B, C.byref(inp), C.byref(out)))
+        ext_args = ()
+        if ext is not None:
+            sc = np.ascontiguousarray(ext[0], dtype=np.uint32) if ext[0] is not None else None
+            nm = np.ascontiguousarray(ext[1], dtype=ft) if ext[1] is not None else None
+            ext_args = (C.byref(InputsExt(_p(sc), _p(nm))),)
+        _check(fn(self.h, B, C.byref(inp), *ext_args, C.byref(out), *warm_args))
         return (f, status, iters, u) if want_u else (f, status, iters)
+
+    def solve(self, st, want_u=False):
+        """host arrays in, host arrays out (H2D + kernels + D2H inside the call)"""
+        return self._solve(lib().a1mpc_solve_batch, st, want_u)
 
     def warm_alloc(self, B):
         """device-resident warm-start state for B robots (no guess yet); free with a1mpc_device_free / Engine.dfree"""
@@ -260,46 +270,16 @@ class Engine:
 
     def solve_warm(self, st, warm, shift=0):
         """a1mpc_solve_batch_warm: host arrays in/out, `warm` from warm_alloc (updated in place on the device)"""
-        B = st["x0"].shape[1]
-        a = {k: np.ascontiguousarray(st[k], dtype=(np.uint32 if k == "contact" else self.ftype)) for k in ("x0", "rot", "foot", "ref", "contact")}
-        f = np.zeros((12, B), dtype=self.ftype); status = np.zeros(B, dtype=np.int32); iters = np.zeros(B, dtype=np.int32)
-        inp = Inputs(_p(a["x0"]), _p(a["rot"]), _p(a["foot"]), _p(a["ref"]), _p(a["contact"]), B)
-        out = Outputs(_p(f), _p(status), _p(iters), None, B)
-        _check(lib().a1mpc_solve_batch_warm(self.h, B, C.byref(inp), C.byref(out), warm, int(shift)))
-        return f, status, iters
+        return self._solve(lib().a1mpc_solve_batch_warm, st, warm_args=(warm, int(shift)))
 
     def solve_ext(self, st, sched=None, normals=None, want_u=False):
         """BASELINE config 4 (extension): per-step contact schedule [N,B] and/or terrain normals [12,B]"""
-        B = st["x0"].shape[1]
-        N = self.cfg.horizon
-        ft = self.ftype
-        a = {k: np.ascontiguousarray(st[k], dtype=(np.uint32 if k == "contact" else ft)) for k in ("x0", "rot", "foot", "ref", "contact")}
-        sc = np.ascontiguousarray(sched, dtype=np.uint32) if sched is not None else None
-        nm = np.ascontiguousarray(normals, dtype=ft) if normals is not None else None
-        f = np.zeros((12, B), dtype=ft); status = np.zeros(B, dtype=np.int32); iters = np.zeros(B, dtype=np.int32)
-        u = np.zeros((12 * N, B), dtype=ft) if want_u else None
-        inp = Inputs(_p(a["x0"]), _p(a["rot"]), _p(a["foot"]), _p(a["ref"]), _p(a["contact"]), B)
-        ext = InputsExt(_p(sc), _p(nm))
-        out = Outputs(_p(f), _p(status), _p(iters), _p(u), B)
-        _check(lib().a1mpc_solve_batch_ext(self.h, B, C.byref(inp), C.byref(ext), C.byref(out)))
-        return (f, status, iters, u) if want_u else (f, status, iters)
+        return self._solve(lib().a1mpc_solve_batch_ext, st, want_u, ext=(sched, normals))
 
     def solve_ext_warm(self, st, sched, normals, warm, shift=1, want_u=False):
         """a1mpc_solve_batch_ext_warm: solve_ext with the device-resident warm start (`warm` from warm_alloc, updated in place);
         shift = 1 for schedules that move one step per control tick (a1mpc_update_plan_batch)"""
-        B = st["x0"].shape[1]
-        N = self.cfg.horizon
-        ft = self.ftype
-        a = {k: np.ascontiguousarray(st[k], dtype=(np.uint32 if k == "contact" else ft)) for k in ("x0", "rot", "foot", "ref", "contact")}
-        sc = np.ascontiguousarray(sched, dtype=np.uint32) if sched is not None else None
-        nm = np.ascontiguousarray(normals, dtype=ft) if normals is not None else None
-        f = np.zeros((12, B), dtype=ft); status = np.zeros(B, dtype=np.int32); iters = np.zeros(B, dtype=np.int32)
-        u = np.zeros((12 * N, B), dtype=ft) if want_u else None
-        inp = Inputs(_p(a["x0"]), _p(a["rot"]), _p(a["foot"]), _p(a["ref"]), _p(a["contact"]), B)
-        ext = InputsExt(_p(sc), _p(nm))
-        out = Outputs(_p(f), _p(status), _p(iters), _p(u), B)
-        _check(lib().a1mpc_solve_batch_ext_warm(self.h, B, C.byref(inp), C.byref(ext), C.byref(out), warm, int(shift)))
-        return (f, status, iters, u) if want_u else (f, status, iters)
+        return self._solve(lib().a1mpc_solve_batch_ext_warm, st, want_u, ext=(sched, normals), warm_args=(warm, int(shift)))
 
     def solve_ptrs(self, B, inp, out):
         """raw a1mpc_solve_batch on caller-built Inputs/Outputs (host or device pointers)"""

@@ -51,19 +51,11 @@ struct a1mpc_handle {
   bool ext_compact = false;
   double* d_rec_ext = nullptr;
   size_t cap_ext = 0;
-  uint32_t* d_sched = nullptr;
-  double* d_normals = nullptr;
-  size_t cap_ext_mirror = 0;
   // scratch sized for `cap` QPs
   size_t cap = 0;
   double* d_rec = nullptr;
   int* d_count = nullptr;
-  // device mirrors for host-pointer calls
-  double *d_x0 = nullptr, *d_rot = nullptr, *d_foot = nullptr, *d_ref = nullptr, *d_f = nullptr, *d_u = nullptr;
-  uint32_t* d_contact = nullptr;
-  int32_t *d_status = nullptr, *d_iters = nullptr;
-  size_t cap_u = 0;
-  // generic scratch for the QP-major side APIs
+  // device copies of the batch arrays of a host-pointer call (Stage)
   void* d_side = nullptr;
   size_t side_bytes = 0;
   int* d_lists = nullptr;
@@ -96,35 +88,15 @@ struct a1mpc_handle {
 
 namespace {
 
-int ensure_capacity(a1mpc_handle* h, size_t B, bool mirrors, bool want_u) {
+int ensure_capacity(a1mpc_handle* h, size_t B) {
   if (B > h->cap) {
     CK(cudaStreamSynchronize(h->stream));
-    auto fr = [](void* p) { if (p) cudaFree(p); };
-    fr(h->d_rec); fr(h->d_x0); fr(h->d_rot); fr(h->d_foot); fr(h->d_ref); fr(h->d_f); fr(h->d_contact); fr(h->d_status); fr(h->d_iters);
-    fr(h->d_u);
-    h->d_rec = h->d_x0 = h->d_rot = h->d_foot = h->d_ref = h->d_f = h->d_u = nullptr;
-    h->d_contact = nullptr; h->d_status = h->d_iters = nullptr;
-    h->cap_u = 0;
+    if (h->d_rec) cudaFree(h->d_rec);
+    h->d_rec = nullptr;
     size_t cap = 1024;
     while (cap < B) cap *= 2;
     h->cap = cap;
     CK(cudaMalloc(&h->d_rec, 4 * cap * REC_BYTES));
-  }
-  if (mirrors && !h->d_x0) {
-    const size_t cap = h->cap;
-    CK(cudaMalloc(&h->d_x0, 12 * cap * 8));
-    CK(cudaMalloc(&h->d_rot, 9 * cap * 8));
-    CK(cudaMalloc(&h->d_foot, 12 * cap * 8));
-    CK(cudaMalloc(&h->d_ref, 9 * cap * 8));
-    CK(cudaMalloc(&h->d_f, 12 * cap * 8));
-    CK(cudaMalloc(&h->d_contact, cap * 4));
-    CK(cudaMalloc(&h->d_status, cap * 4));
-    CK(cudaMalloc(&h->d_iters, cap * 4));
-  }
-  if (mirrors && want_u && h->cap_u < h->cap) {
-    if (h->d_u) cudaFree(h->d_u);
-    CK(cudaMalloc(&h->d_u, (size_t)12 * h->cfg.horizon * h->cap * 8));
-    h->cap_u = h->cap;
   }
   return A1MPC_OK;
 }
@@ -161,13 +133,102 @@ bool is_device_ptr(const void* p) {
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
-// true when the non-NULL pointers do not all live on the same side as `dev` says (a host pointer dereferenced by a kernel is a sticky
-// fault for the whole CUDA context, so every entry point classifies every array it is given)
-bool mixed_sides(bool dev, std::initializer_list<const void*> ptrs) {
-  for (const void* q : ptrs)
-    if (q && is_device_ptr(q) != dev) return true;
-  return false;
-}
+// The one path by which the batch arrays of an entry point reach its kernels.  The call declares each array (in, out or in/out:
+// rows x B elements of 4 or 8 bytes, leading dimension ld in the caller's memory), then begin() classifies every non-NULL array
+// once: they must all be host or all device memory, because a host pointer dereferenced by a kernel is a sticky fault for the
+// whole CUDA context.  A mix is rejected before anything is enqueued, and so is a device pointer among the batch-uniform
+// parameters that the call reads on the host.  Device arrays go to the kernel as they are and the call stays asynchronous.
+// Host arrays get one dense [rows][B] slot each in h->d_side: begin() copies the inputs in and points the call's variable at the
+// slot, finish() copies the outputs back and synchronises the stream once.
+class Stage {
+ public:
+  Stage(a1mpc_handle* h, int B) : h_(h), B_((size_t)B) { arrays_.reserve(16); }   // update_plan declares the most: 15
+  template <class T> void in(T*& p, size_t rows, size_t esz = sizeof(T)) { add(p, IN, rows, esz, B_); }
+  template <class T> void in(T*& p, size_t rows, size_t esz, size_t ld) { add(p, IN, rows, esz, ld); }
+  template <class T> void out(T*& p, size_t rows, size_t esz = sizeof(T)) { add(p, OUT, rows, esz, B_); }
+  template <class T> void out(T*& p, size_t rows, size_t esz, size_t ld) { add(p, OUT, rows, esz, ld); }
+  template <class T> void inout(T*& p, size_t rows, size_t esz = sizeof(T)) { add(p, INOUT, rows, esz, B_); }
+  // a batch array this call does not read: its side is checked, nothing is copied
+  void unused(const void* p) { arrays_.push_back({nullptr, nullptr, const_cast<void*>(p), 0, 0, 0, UNUSED, nullptr}); }
+  // a batch-uniform parameter read by the call itself on the host
+  void host_param(const void* p, const char* name) { params_.push_back({p, name}); }
+  bool host() const { return host_; }
+
+  int begin() {
+    bool first = true;
+    for (const Array& a : arrays_) {
+      if (!a.user) continue;
+      const bool host = !is_device_ptr(a.user);
+      if (first) {
+        host_ = host;
+        first = false;
+      } else if (host != host_) {
+        return fail(A1MPC_EINVAL, "batch arrays must be all-host or all-device");
+      }
+    }
+    for (const Param& p : params_)
+      if (is_device_ptr(p.ptr)) return fail(A1MPC_EINVAL, std::string(p.name) + " must be a host array (batch-uniform parameter)");
+    if (!host_) return A1MPC_OK;
+    size_t bytes = 0;
+    for (const Array& a : arrays_)
+      if (a.user && a.dir != UNUSED) bytes += pad(a.rows * B_ * a.esz);
+    int rc;
+    if ((rc = ensure_side(h_, bytes))) return rc;
+    char* cur = static_cast<char*>(h_->d_side);
+    for (Array& a : arrays_) {
+      if (!a.user || a.dir == UNUSED) continue;
+      a.slot = cur;
+      cur += pad(a.rows * B_ * a.esz);
+      a.point(a.var, a.slot);
+      if (a.dir != OUT && (rc = copy(a, cudaMemcpyHostToDevice))) return rc;
+    }
+    return A1MPC_OK;
+  }
+
+  int finish() {
+    if (!host_) return A1MPC_OK;
+    int rc;
+    for (const Array& a : arrays_)
+      if (a.user && (a.dir == OUT || a.dir == INOUT) && (rc = copy(a, cudaMemcpyDeviceToHost))) return rc;
+    CK(cudaStreamSynchronize(h_->stream));
+    return A1MPC_OK;
+  }
+
+ private:
+  enum Dir { IN, OUT, INOUT, UNUSED };
+  struct Array {
+    void* var;                     // the call's pointer variable, pointed at the slot in host mode
+    void (*point)(void*, char*);
+    void* user;                    // the caller's array
+    size_t rows, esz, ld;
+    Dir dir;
+    char* slot;
+  };
+  struct Param { const void* ptr; const char* name; };
+  static size_t pad(size_t b) { return (b + 255) & ~(size_t)255; }
+
+  template <class T>
+  void add(T*& p, Dir dir, size_t rows, size_t esz, size_t ld) {
+    arrays_.push_back({&p, [](void* var, char* slot) { *static_cast<T**>(var) = reinterpret_cast<T*>(slot); },
+                       const_cast<void*>(static_cast<const void*>(p)), rows, esz, ld, dir, nullptr});
+  }
+
+  int copy(const Array& a, cudaMemcpyKind kind) {
+    const bool h2d = kind == cudaMemcpyHostToDevice;
+    void* dst = h2d ? a.slot : a.user;
+    const void* src = h2d ? a.user : a.slot;
+    const size_t row = B_ * a.esz, user_pitch = a.ld * a.esz;
+    if (a.ld == B_) CK(cudaMemcpyAsync(dst, src, a.rows * row, kind, h_->stream));
+    else CK(cudaMemcpy2DAsync(dst, h2d ? row : user_pitch, src, h2d ? user_pitch : row, row, a.rows, kind, h_->stream));
+    return A1MPC_OK;
+  }
+
+  a1mpc_handle* h_;
+  size_t B_;
+  bool host_ = false;
+  std::vector<Array> arrays_;
+  std::vector<Param> params_;
+};
 
 // enqueue the fused path on device-resident SoA data
 void attach_peers(a1mpc_handle* h, int B, DevOutputs& d) {
@@ -220,9 +281,82 @@ int enqueue_solve(a1mpc_handle* h, int B, const DevInputs& din, const DevOutputs
   return peer_signal(h, B);   // fused collect: publish this call's step number to every rank (no-op when not connected)
 }
 
-int copy_rows(cudaStream_t st, void* dst, size_t dst_ld, const void* src, size_t src_ld, int rows, size_t B, size_t esz, cudaMemcpyKind kind) {
-  CK(cudaMemcpy2DAsync(dst, dst_ld * esz, src, src_ld * esz, B * esz, rows, kind, st));
+// the same on a schedule (dsched) and / or terrain normals (dnorm): a1mpc_solve_batch_ext and _ext_warm
+int enqueue_solve_ext(a1mpc_handle* h, int B, const DevInputs& di, const uint32_t* dsched, const double* dnorm, const DevOutputs& dout_in,
+                      uint32_t* warm, int shift) {
+  const int N = h->cfg.horizon;
+  if ((size_t)B > h->cap_ext) {
+    CK(cudaStreamSynchronize(h->stream));
+    if (h->d_rec_ext) cudaFree(h->d_rec_ext);
+    h->d_rec_ext = nullptr;
+    CK(cudaMalloc(&h->d_rec_ext, 2 * h->cap * REC_EXT_BYTES));   // second half: queue of the compacted class
+    h->cap_ext = h->cap;
+  }
+  DevOutputs dout = dout_in;
+  attach_peers(h, -1, dout);   // the fused collect is wired to a1mpc_solve_batch / _warm only
+  CK(cudaMemsetAsync(h->d_count, 0, 16 * sizeof(int), h->stream));
+  if (warm) {   // robots without any contact are answered by the pack kernel and store no guess
+    warm_forget_no_contact_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, B, warm, N);
+    h->launches++;
+  }
+  if (h->ext_compact && dsched) {
+    pack_ext2_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, (int)h->cap_ext, h->d_count, dout, N);
+    const double* rec2 = h->d_rec_ext + h->cap_ext * REC_EXT_DOUBLES;
+    if (warm) {
+      ext_warm_launch(h->cls_ext_warm, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout, warm, shift);
+      sched2_warm_launch(h->cls_sched2_warm, h->stream, B, h->P, rec2, h->d_count, dout, warm, shift);
+    } else {
+      ext_launch(N, h->cls_ext, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout);
+      sched2_launch(h->cls_sched2, h->stream, B, h->P, rec2, h->d_count, dout);
+    }
+    h->launches += 3;
+  } else {
+    pack_ext_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, h->d_count, dout, N);
+    if (warm) ext_warm_launch(h->cls_ext_warm, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout, warm, shift);
+    else ext_launch(N, h->cls_ext, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout);
+    h->launches += 2;
+  }
+  CK(cudaGetLastError());
   return A1MPC_OK;
+}
+
+// a1mpc_solve_batch, _warm, _ext and _ext_warm.  ext: schedule and / or normals (NULL, or both fields NULL: the plain solve);
+// warm_start: the _warm calls, with the caller's `warm` buffer and `shift`
+int solve_impl(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_inputs_ext* ext, const a1mpc_outputs* out, bool warm_start,
+               void* warm, int shift) {
+  if (!h || !in || !out || (warm_start && !warm)) return fail(A1MPC_EINVAL, "null argument");
+  if (ext && !ext->contact_sched && !ext->normals) ext = nullptr;
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (!in->x0 || !in->rot || !in->foot || !in->ref || !in->contact || !out->f_body || !out->status) return fail(A1MPC_EINVAL, "null input/output array");
+  if (in->ld < (size_t)B || out->ld < (size_t)B) return fail(A1MPC_EINVAL, "ld < B");
+  const int N = h->cfg.horizon;
+  if (warm_start && N != 10) return fail(A1MPC_EINVAL, "warm start is implemented for horizon 10 (see include/a1mpc.h)");
+  if (warm_start && (shift < 0 || shift > N)) return fail(A1MPC_EINVAL, "shift out of range");
+  if (ext && ext->normals)
+    for (int i = 0; i < 4; ++i)
+      if (h->cfg.r[3 * i] != h->cfg.r[3 * i + 1] || h->cfg.r[3 * i] != h->cfg.r[3 * i + 2])
+        return fail(A1MPC_EINVAL, "terrain normals need isotropic r weights per foot (r[3i] == r[3i+1] == r[3i+2])");
+  CK(cudaSetDevice(h->device));
+  if (warm_start && !is_device_ptr(warm)) return fail(A1MPC_EINVAL, "warm must be device memory (a1mpc_device_alloc)");
+  const int f32 = (h->cfg.precision == 32) ? 1 : 0;   // fp32 arrays at the boundary, fp64 inside
+  const size_t es = f32 ? 4 : 8;
+  DevInputs di{in->x0, in->rot, in->foot, in->ref, in->contact, in->ld, f32};
+  DevOutputs dout{out->f_body, out->status, out->iters, out->u_full, out->ld, f32};
+  const uint32_t* dsched = ext ? ext->contact_sched : nullptr;
+  const double* dnorm = ext ? ext->normals : nullptr;
+  Stage st(h, B);
+  st.in(di.x0, 12, es, in->ld); st.in(di.rot, 9, es, in->ld); st.in(di.foot, 12, es, in->ld); st.in(di.ref, 9, es, in->ld);
+  st.in(di.contact, 1);
+  st.in(dsched, N, 4, in->ld); st.in(dnorm, 12, es, in->ld);
+  st.out(dout.f_body, 12, es, out->ld); st.out(dout.status, 1); st.out(dout.iters, 1); st.out(dout.u_full, 12 * N, es, out->ld);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  if (st.host()) di.ld = dout.ld = (size_t)B;
+  if ((rc = ensure_capacity(h, B))) return rc;
+  uint32_t* w = static_cast<uint32_t*>(warm);
+  rc = ext ? enqueue_solve_ext(h, B, di, dsched, dnorm, dout, w, shift) : enqueue_solve(h, B, di, dout, w, shift);
+  if (rc) return rc;
+  return st.finish();
 }
 
 }  // namespace
@@ -341,9 +475,7 @@ int a1mpc_destroy(a1mpc_handle* h) {
   if (h->nccl_comm) { a1mpc_internal_nccl_destroy(h->nccl_comm); h->nccl_comm = nullptr; }   // before its streams go away
   a1mpc_peer_gather_destroy(h);
   auto fr = [](void* p) { if (p) cudaFree(p); };
-  fr(h->d_rec); fr(h->d_count); fr(h->d_x0); fr(h->d_rot); fr(h->d_foot); fr(h->d_ref); fr(h->d_f); fr(h->d_u);
-  fr(h->d_contact); fr(h->d_status); fr(h->d_iters); fr(h->d_side); fr(h->d_flush); fr(h->d_lists);
-  fr(h->d_rec_ext); fr(h->d_sched); fr(h->d_normals);
+  fr(h->d_rec); fr(h->d_count); fr(h->d_side); fr(h->d_flush); fr(h->d_lists); fr(h->d_rec_ext);
   for (int i = 0; i < 4; ++i) {
     if (h->side[i]) cudaStreamDestroy(h->side[i]);
     if (h->ev_join[i]) cudaEventDestroy(h->ev_join[i]);
@@ -356,47 +488,9 @@ int a1mpc_destroy(a1mpc_handle* h) {
   return A1MPC_OK;
 }
 
-static int solve_batch_impl(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_outputs* out, uint32_t* warm, int shift) {
-  if (!h || !in || !out) return fail(A1MPC_EINVAL, "null argument");
-  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
-  if (!in->x0 || !in->rot || !in->foot || !in->ref || !in->contact || !out->f_body || !out->status) return fail(A1MPC_EINVAL, "null input/output array");
-  if (in->ld < (size_t)B || out->ld < (size_t)B) return fail(A1MPC_EINVAL, "ld < B");
-  CK(cudaSetDevice(h->device));
-  // every array of the call lives on the same side (a host pointer dereferenced by a kernel is a sticky fault for the whole context)
-  const bool dev_in = is_device_ptr(in->x0), dev_out = is_device_ptr(out->f_body);
-  const void* all_ptrs[] = {in->rot, in->foot, in->ref, in->contact, out->status, out->iters, out->u_full};
-  bool mixed = (dev_in != dev_out);
-  for (const void* q : all_ptrs) mixed = mixed || (q && is_device_ptr(q) != dev_in);
-  if (mixed) return fail(A1MPC_EINVAL, "inputs and outputs must be all-host or all-device");
-  const int f32 = (h->cfg.precision == 32) ? 1 : 0;   // fp32 arrays at the boundary, fp64 inside
-  const size_t es = f32 ? 4 : 8;
-  int rc;
-  if (dev_in) {
-    if ((rc = ensure_capacity(h, B, false, false))) return rc;
-    DevInputs di{in->x0, in->rot, in->foot, in->ref, in->contact, in->ld, f32};
-    DevOutputs dout{out->f_body, out->status, out->iters, out->u_full, out->ld, f32};
-    return enqueue_solve(h, B, di, dout, warm, shift);
-  }
-  if ((rc = ensure_capacity(h, B, true, out->u_full != nullptr))) return rc;
-  const size_t Bs = (size_t)B;
-  if ((rc = copy_rows(h->stream, h->d_x0, Bs, in->x0, in->ld, 12, Bs, es, cudaMemcpyHostToDevice))) return rc;
-  if ((rc = copy_rows(h->stream, h->d_rot, Bs, in->rot, in->ld, 9, Bs, es, cudaMemcpyHostToDevice))) return rc;
-  if ((rc = copy_rows(h->stream, h->d_foot, Bs, in->foot, in->ld, 12, Bs, es, cudaMemcpyHostToDevice))) return rc;
-  if ((rc = copy_rows(h->stream, h->d_ref, Bs, in->ref, in->ld, 9, Bs, es, cudaMemcpyHostToDevice))) return rc;
-  CK(cudaMemcpyAsync(h->d_contact, in->contact, Bs * 4, cudaMemcpyHostToDevice, h->stream));
-  DevInputs di{h->d_x0, h->d_rot, h->d_foot, h->d_ref, h->d_contact, Bs, f32};
-  DevOutputs dout{h->d_f, h->d_status, out->iters ? h->d_iters : nullptr, out->u_full ? h->d_u : nullptr, Bs, f32};
-  if ((rc = enqueue_solve(h, B, di, dout, warm, shift))) return rc;
-  if ((rc = copy_rows(h->stream, out->f_body, out->ld, h->d_f, Bs, 12, Bs, es, cudaMemcpyDeviceToHost))) return rc;
-  CK(cudaMemcpyAsync(out->status, h->d_status, Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (out->iters) CK(cudaMemcpyAsync(out->iters, h->d_iters, Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (out->u_full)
-    if ((rc = copy_rows(h->stream, out->u_full, out->ld, h->d_u, Bs, 12 * h->cfg.horizon, Bs, es, cudaMemcpyDeviceToHost))) return rc;
-  CK(cudaStreamSynchronize(h->stream));
-  return A1MPC_OK;
+int a1mpc_solve_batch(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_outputs* out) {
+  return solve_impl(h, B, in, nullptr, out, false, nullptr, 0);
 }
-
-int a1mpc_solve_batch(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_outputs* out) { return solve_batch_impl(h, B, in, out, nullptr, 0); }
 
 size_t a1mpc_warm_bytes(const a1mpc_handle* h, int B) {
   if (!h || B <= 0) return 0;
@@ -412,168 +506,39 @@ int a1mpc_warm_reset(a1mpc_handle* h, void* warm, int B) {
 }
 
 int a1mpc_solve_batch_warm(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_outputs* out, void* warm, int shift) {
-  if (!h || !warm) return fail(A1MPC_EINVAL, "null argument");
-  if (h->cfg.horizon != 10) return fail(A1MPC_EINVAL, "warm start is implemented for horizon 10 (see include/a1mpc.h)");
-  if (shift < 0 || shift > h->cfg.horizon) return fail(A1MPC_EINVAL, "shift out of range");
-  CK(cudaSetDevice(h->device));
-  if (!is_device_ptr(warm)) return fail(A1MPC_EINVAL, "warm must be device memory (a1mpc_device_alloc)");
-  return solve_batch_impl(h, B, in, out, static_cast<uint32_t*>(warm), shift);
-}
-
-// a1mpc_solve_batch_ext (warm == nullptr) and a1mpc_solve_batch_ext_warm; ext carries a schedule and / or normals
-static int solve_ext_impl(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_inputs_ext* ext, const a1mpc_outputs* out, uint32_t* warm,
-                          int shift) {
-  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
-  if (!in->x0 || !in->rot || !in->foot || !in->ref || !in->contact || !out->f_body || !out->status) return fail(A1MPC_EINVAL, "null input/output array");
-  if (in->ld < (size_t)B || out->ld < (size_t)B) return fail(A1MPC_EINVAL, "ld < B");
-  if (ext->normals)
-    for (int i = 0; i < 4; ++i)
-      if (h->cfg.r[3 * i] != h->cfg.r[3 * i + 1] || h->cfg.r[3 * i] != h->cfg.r[3 * i + 2])
-        return fail(A1MPC_EINVAL, "terrain normals need isotropic r weights per foot (r[3i] == r[3i+1] == r[3i+2])");
-  CK(cudaSetDevice(h->device));
-  const int N = h->cfg.horizon;
-  const size_t Bs = (size_t)B;
-  const bool dev = is_device_ptr(in->x0);
-  {
-    const void* all_ptrs[] = {in->rot, in->foot, in->ref, in->contact, out->f_body, out->status, out->iters, out->u_full, ext->contact_sched, ext->normals};
-    for (const void* q : all_ptrs)
-      if (q && is_device_ptr(q) != dev) return fail(A1MPC_EINVAL, "inputs and outputs must be all-host or all-device");
-  }
-  const int f32 = (h->cfg.precision == 32) ? 1 : 0;
-  const size_t es = f32 ? 4 : 8;
-  int rc;
-  if ((rc = ensure_capacity(h, B, !dev, !dev && out->u_full != nullptr))) return rc;
-  if (Bs > h->cap_ext) {
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->d_rec_ext) cudaFree(h->d_rec_ext);
-    h->d_rec_ext = nullptr;
-    CK(cudaMalloc(&h->d_rec_ext, 2 * h->cap * REC_EXT_BYTES));   // second half: queue of the compacted class
-    h->cap_ext = h->cap;
-  }
-  DevInputs di{in->x0, in->rot, in->foot, in->ref, in->contact, in->ld, f32};
-  DevOutputs dout{out->f_body, out->status, out->iters, out->u_full, out->ld, f32};
-  const uint32_t* dsched = ext->contact_sched;
-  const double* dnorm = ext->normals;
-  if (!dev) {
-    if (Bs > h->cap_ext_mirror) {
-      CK(cudaStreamSynchronize(h->stream));
-      if (h->d_sched) cudaFree(h->d_sched);
-      if (h->d_normals) cudaFree(h->d_normals);
-      h->d_sched = nullptr; h->d_normals = nullptr;
-      CK(cudaMalloc(&h->d_sched, (size_t)A1MPC_MAX_HORIZON * h->cap * 4));
-      CK(cudaMalloc(&h->d_normals, 12 * h->cap * 8));
-      h->cap_ext_mirror = h->cap;
-    }
-    if ((rc = copy_rows(h->stream, h->d_x0, Bs, in->x0, in->ld, 12, Bs, es, cudaMemcpyHostToDevice))) return rc;
-    if ((rc = copy_rows(h->stream, h->d_rot, Bs, in->rot, in->ld, 9, Bs, es, cudaMemcpyHostToDevice))) return rc;
-    if ((rc = copy_rows(h->stream, h->d_foot, Bs, in->foot, in->ld, 12, Bs, es, cudaMemcpyHostToDevice))) return rc;
-    if ((rc = copy_rows(h->stream, h->d_ref, Bs, in->ref, in->ld, 9, Bs, es, cudaMemcpyHostToDevice))) return rc;
-    CK(cudaMemcpyAsync(h->d_contact, in->contact, Bs * 4, cudaMemcpyHostToDevice, h->stream));
-    if (ext->contact_sched) {
-      if ((rc = copy_rows(h->stream, h->d_sched, Bs, ext->contact_sched, in->ld, N, Bs, 4, cudaMemcpyHostToDevice))) return rc;
-      dsched = h->d_sched;
-    }
-    if (ext->normals) {
-      if ((rc = copy_rows(h->stream, h->d_normals, Bs, ext->normals, in->ld, 12, Bs, es, cudaMemcpyHostToDevice))) return rc;
-      dnorm = h->d_normals;
-    }
-    di = DevInputs{h->d_x0, h->d_rot, h->d_foot, h->d_ref, h->d_contact, Bs, f32};
-    dout = DevOutputs{h->d_f, h->d_status, out->iters ? h->d_iters : nullptr, out->u_full ? h->d_u : nullptr, Bs, f32};
-  }
-  attach_peers(h, -1, dout);   // the fused collect is wired to a1mpc_solve_batch / _warm only
-  CK(cudaMemsetAsync(h->d_count, 0, 16 * sizeof(int), h->stream));
-  if (warm) {   // robots without any contact are answered by the pack kernel and store no guess
-    warm_forget_no_contact_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, B, warm, N);
-    h->launches++;
-  }
-  if (h->ext_compact && dsched) {
-    pack_ext2_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, (int)h->cap_ext, h->d_count, dout, N);
-    const double* rec2 = h->d_rec_ext + h->cap_ext * REC_EXT_DOUBLES;
-    if (warm) {
-      ext_warm_launch(h->cls_ext_warm, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout, warm, shift);
-      sched2_warm_launch(h->cls_sched2_warm, h->stream, B, h->P, rec2, h->d_count, dout, warm, shift);
-    } else {
-      ext_launch(N, h->cls_ext, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout);
-      sched2_launch(h->cls_sched2, h->stream, B, h->P, rec2, h->d_count, dout);
-    }
-    h->launches += 3;
-  } else {
-    pack_ext_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, h->d_count, dout, N);
-    if (warm) ext_warm_launch(h->cls_ext_warm, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout, warm, shift);
-    else ext_launch(N, h->cls_ext, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout);
-    h->launches += 2;
-  }
-  CK(cudaGetLastError());
-  if (!dev) {
-    if ((rc = copy_rows(h->stream, out->f_body, out->ld, h->d_f, Bs, 12, Bs, es, cudaMemcpyDeviceToHost))) return rc;
-    CK(cudaMemcpyAsync(out->status, h->d_status, Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-    if (out->iters) CK(cudaMemcpyAsync(out->iters, h->d_iters, Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-    if (out->u_full)
-      if ((rc = copy_rows(h->stream, out->u_full, out->ld, h->d_u, Bs, 12 * N, Bs, es, cudaMemcpyDeviceToHost))) return rc;
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return A1MPC_OK;
+  return solve_impl(h, B, in, nullptr, out, true, warm, shift);
 }
 
 int a1mpc_solve_batch_ext(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_inputs_ext* ext, const a1mpc_outputs* out) {
-  if (!h || !in || !out) return fail(A1MPC_EINVAL, "null argument");
-  if (!ext || (!ext->contact_sched && !ext->normals)) return a1mpc_solve_batch(h, B, in, out);
-  return solve_ext_impl(h, B, in, ext, out, nullptr, 0);
+  return solve_impl(h, B, in, ext, out, false, nullptr, 0);
 }
 
 int a1mpc_solve_batch_ext_warm(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_inputs_ext* ext, const a1mpc_outputs* out, void* warm,
                                int shift) {
-  if (!h || !in || !out || !warm) return fail(A1MPC_EINVAL, "null argument");
-  if (!ext || (!ext->contact_sched && !ext->normals)) return a1mpc_solve_batch_warm(h, B, in, out, warm, shift);
-  if (h->cfg.horizon != 10) return fail(A1MPC_EINVAL, "warm start is implemented for horizon 10 (see include/a1mpc.h)");
-  if (shift < 0 || shift > h->cfg.horizon) return fail(A1MPC_EINVAL, "shift out of range");
-  CK(cudaSetDevice(h->device));
-  if (!is_device_ptr(warm)) return fail(A1MPC_EINVAL, "warm must be device memory (a1mpc_device_alloc)");
-  return solve_ext_impl(h, B, in, ext, out, static_cast<uint32_t*>(warm), shift);
+  return solve_impl(h, B, in, ext, out, true, warm, shift);
 }
 
 int a1mpc_build_qp_batch(a1mpc_handle* h, int B, const a1mpc_inputs* in, double* H, double* g, double* lb, double* ub) {
   if (!h || !in) return fail(A1MPC_EINVAL, "null argument");
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (!in->x0 || !in->rot || !in->foot || !in->ref || !in->contact) return fail(A1MPC_EINVAL, "null input array");
   if ((lb == nullptr) != (ub == nullptr)) return fail(A1MPC_EINVAL, "lb and ub must be given together");
   CK(cudaSetDevice(h->device));
   const int N = h->cfg.horizon, n = 12 * N, m = 20 * N;
-  const bool dev = is_device_ptr(in->x0);
-  if (mixed_sides(dev, {in->rot, in->foot, in->ref, in->contact, H, g, lb, ub})) return fail(A1MPC_EINVAL, "inputs and outputs must be all-host or all-device");
-  int rc;
   DevInputs di{in->x0, in->rot, in->foot, in->ref, in->contact, in->ld};
-  double *dH = H, *dg = g, *dlb = lb, *dub = ub;
-  if (!dev) {
-    if ((rc = ensure_capacity(h, B, true, false))) return rc;
-    const size_t Bs = (size_t)B;
-    if ((rc = copy_rows(h->stream, h->d_x0, Bs, in->x0, in->ld, 12, Bs, 8, cudaMemcpyHostToDevice))) return rc;
-    if ((rc = copy_rows(h->stream, h->d_rot, Bs, in->rot, in->ld, 9, Bs, 8, cudaMemcpyHostToDevice))) return rc;
-    if ((rc = copy_rows(h->stream, h->d_foot, Bs, in->foot, in->ld, 12, Bs, 8, cudaMemcpyHostToDevice))) return rc;
-    if ((rc = copy_rows(h->stream, h->d_ref, Bs, in->ref, in->ld, 9, Bs, 8, cudaMemcpyHostToDevice))) return rc;
-    CK(cudaMemcpyAsync(h->d_contact, in->contact, Bs * 4, cudaMemcpyHostToDevice, h->stream));
-    di = DevInputs{h->d_x0, h->d_rot, h->d_foot, h->d_ref, h->d_contact, Bs};
-    const size_t bytes = Bs * ((size_t)n * n + n + 2 * m) * 8;
-    if ((rc = ensure_side(h, bytes))) return rc;
-    double* base = (double*)h->d_side;
-    dH = H ? base : nullptr;
-    dg = g ? base + Bs * n * n : nullptr;
-    dlb = lb ? base + Bs * n * n + Bs * n : nullptr;
-    dub = ub ? base + Bs * n * n + Bs * n + Bs * m : nullptr;
-  }
+  Stage st(h, B);
+  st.in(di.x0, 12, 8, in->ld); st.in(di.rot, 9, 8, in->ld); st.in(di.foot, 12, 8, in->ld); st.in(di.ref, 9, 8, in->ld);
+  st.in(di.contact, 1);
+  st.out(H, (size_t)n * n); st.out(g, n); st.out(lb, m); st.out(ub, m);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  if (st.host()) di.ld = (size_t)B;
   {
-    cudaError_t e = build_dense_launch(h->P, di, B, dH, dg, dlb, dub, h->stream);
+    cudaError_t e = build_dense_launch(h->P, di, B, H, g, lb, ub, h->stream);
     if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("build kernel: ") + cudaGetErrorString(e));
     h->launches++;
   }
-  if (!dev) {
-    const size_t Bs = (size_t)B;
-    if (H) CK(cudaMemcpyAsync(H, dH, Bs * n * n * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (g) CK(cudaMemcpyAsync(g, dg, Bs * n * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (lb) CK(cudaMemcpyAsync(lb, dlb, Bs * m * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (ub) CK(cudaMemcpyAsync(ub, dub, Bs * m * 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return A1MPC_OK;
+  return st.finish();
 }
 
 static int qp_mats_impl(a1mpc_handle* h, int B, const double* A_d, const double* B_d_list, const double* x0, const double* x_d,
@@ -582,43 +547,17 @@ static int qp_mats_impl(a1mpc_handle* h, int B, const double* A_d, const double*
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
   CK(cudaSetDevice(h->device));
   const int N = h->cfg.horizon, n = 12 * N;
-  const bool dev = is_device_ptr(A_d);
-  {
-    const void* all_ptrs[] = {B_d_list, x0, x_d, H, g, A_qp, B_qp};
-    for (const void* q : all_ptrs)
-      if (q && is_device_ptr(q) != dev) return fail(A1MPC_EINVAL, "inputs and outputs must be all-host or all-device");
-  }
-  const size_t Bs = (size_t)B;
-  const size_t szA = Bs * 169, szB = Bs * 13 * N * 12, szx0 = Bs * 13, szxd = Bs * 13 * N, szH = H ? Bs * n * n : 0, szg = g ? Bs * n : 0;
-  const size_t szAq = A_qp ? Bs * 13 * N * 13 : 0, szBq = B_qp ? Bs * 13 * N * n : 0;
-  const double *dA = A_d, *dB = B_d_list, *dx0 = x0, *dxd = x_d;
-  double *dH = H, *dg = g, *dAq = A_qp, *dBq = B_qp;
+  Stage st(h, B);
+  st.in(A_d, 169); st.in(B_d_list, 13 * N * 12); st.in(x0, 13); st.in(x_d, 13 * N);
+  st.out(H, (size_t)n * n); st.out(g, n); st.out(A_qp, 13 * N * 13); st.out(B_qp, 13 * N * n);
   int rc;
-  if (!dev) {
-    if ((rc = ensure_side(h, (szA + szB + szx0 + szxd + szH + szg + szAq + szBq) * 8))) return rc;
-    double* p = (double*)h->d_side;
-    CK(cudaMemcpyAsync(p, A_d, szA * 8, cudaMemcpyHostToDevice, h->stream)); dA = p; p += szA;
-    CK(cudaMemcpyAsync(p, B_d_list, szB * 8, cudaMemcpyHostToDevice, h->stream)); dB = p; p += szB;
-    CK(cudaMemcpyAsync(p, x0, szx0 * 8, cudaMemcpyHostToDevice, h->stream)); dx0 = p; p += szx0;
-    CK(cudaMemcpyAsync(p, x_d, szxd * 8, cudaMemcpyHostToDevice, h->stream)); dxd = p; p += szxd;
-    if (H) { dH = p; p += szH; }
-    if (g) { dg = p; p += szg; }
-    if (A_qp) { dAq = p; p += szAq; }
-    if (B_qp) { dBq = p; p += szBq; }
-  }
+  if ((rc = st.begin())) return rc;
   {
-    cudaError_t e = dense_qp_mats_launch(h->P, B, dA, dB, dx0, dxd, dH, dg, dAq, dBq, h->stream);
+    cudaError_t e = dense_qp_mats_launch(h->P, B, A_d, B_d_list, x0, x_d, H, g, A_qp, B_qp, h->stream);
     if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("qp_mats kernel: ") + cudaGetErrorString(e));
     h->launches += 1;
   }
-  if (!dev) {
-    if (H) CK(cudaMemcpyAsync(H, dH, szH * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (g) CK(cudaMemcpyAsync(g, dg, szg * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (A_qp) CK(cudaMemcpyAsync(A_qp, dAq, szAq * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (B_qp) CK(cudaMemcpyAsync(B_qp, dBq, szBq * 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return A1MPC_OK;
+  return st.finish();
 }
 
 int a1mpc_qp_mats_batch(a1mpc_handle* h, int B, const double* A_d, const double* B_d_list, const double* x0, const double* x_d,
@@ -637,39 +576,19 @@ int a1mpc_solve_dense_batch(a1mpc_handle* h, int B, const double* H, const doubl
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
   CK(cudaSetDevice(h->device));
   const int N = h->cfg.horizon, n = 12 * N;
-  const bool dev = is_device_ptr(H);
-  if (mixed_sides(dev, {g, contact, u, status})) return fail(A1MPC_EINVAL, "inputs and outputs must be all-host or all-device");
-  const size_t Bs = (size_t)B;
-  const double *dH = H, *dg = g;
-  const uint32_t* dc = contact;
-  double* du = u;
-  int32_t* ds = status;
+  Stage st(h, B);
+  st.in(H, (size_t)n * n); st.in(g, n); st.in(contact, 1);
+  st.out(u, n); st.out(status, 1);
   int rc;
-  const size_t list_bytes = (4 * Bs + 8) * sizeof(int);
-  if ((rc = ensure_lists(h, list_bytes))) return rc;
-  if (!dev) {
-    const size_t bytes = (Bs * n * n + 2 * Bs * n) * 8 + Bs * 8;
-    if ((rc = ensure_side(h, bytes))) return rc;
-    double* p = (double*)h->d_side;
-    CK(cudaMemcpyAsync(p, H, Bs * n * n * 8, cudaMemcpyHostToDevice, h->stream)); dH = p; p += Bs * n * n;
-    CK(cudaMemcpyAsync(p, g, Bs * n * 8, cudaMemcpyHostToDevice, h->stream)); dg = p; p += Bs * n;
-    du = p; p += Bs * n;
-    uint32_t* pc = (uint32_t*)p;
-    CK(cudaMemcpyAsync(pc, contact, Bs * 4, cudaMemcpyHostToDevice, h->stream)); dc = pc;
-    ds = (int32_t*)(pc + Bs);
-  }
+  if ((rc = st.begin())) return rc;
+  if ((rc = ensure_lists(h, (4 * (size_t)B + 8) * sizeof(int)))) return rc;
   {
     int nl = 0;
-    cudaError_t e = dense_solve_launch(h->P, h->sm_count, B, dH, dg, dc, du, ds, h->d_lists, h->stream, &nl);
+    cudaError_t e = dense_solve_launch(h->P, h->sm_count, B, H, g, contact, u, status, h->d_lists, h->stream, &nl);
     if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("dense solve kernels: ") + cudaGetErrorString(e));
     h->launches += nl;
   }
-  if (!dev) {
-    CK(cudaMemcpyAsync(u, du, Bs * n * 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(status, ds, Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return A1MPC_OK;
+  return st.finish();
 }
 
 int a1mpc_grf_qp_batch(a1mpc_handle* h, int B, const double* root_acc, const double* rot_z, const double* rot, const double* foot,
@@ -677,39 +596,19 @@ int a1mpc_grf_qp_batch(a1mpc_handle* h, int B, const double* root_acc, const dou
   if (!h || !root_acc || !rot_z || !rot || !foot || !contact || !f_body || !status) return fail(A1MPC_EINVAL, "null argument");
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
   CK(cudaSetDevice(h->device));
-  const bool dev = is_device_ptr(root_acc);
-  if (mixed_sides(dev, {rot_z, rot, foot, contact, f_body, status})) return fail(A1MPC_EINVAL, "inputs and outputs must be all-host or all-device");
-  const size_t Bs = (size_t)B;
-  const double *da = root_acc, *drz = rot_z, *dr = rot, *dfo = foot;
-  const uint32_t* dc = contact;
-  double* df = f_body;
-  int32_t* ds = status;
+  Stage st(h, B);
+  st.in(root_acc, 6); st.in(rot_z, 9); st.in(rot, 9); st.in(foot, 12); st.in(contact, 1);
+  st.out(f_body, 12); st.out(status, 1);
   int rc;
-  if ((rc = ensure_lists(h, (4 * Bs + 8) * sizeof(int)))) return rc;
-  if (!dev) {
-    if ((rc = ensure_side(h, Bs * (6 + 9 + 9 + 12 + 12) * 8 + Bs * 8))) return rc;
-    double* p = (double*)h->d_side;
-    CK(cudaMemcpyAsync(p, root_acc, Bs * 6 * 8, cudaMemcpyHostToDevice, h->stream)); da = p; p += Bs * 6;
-    CK(cudaMemcpyAsync(p, rot_z, Bs * 9 * 8, cudaMemcpyHostToDevice, h->stream)); drz = p; p += Bs * 9;
-    CK(cudaMemcpyAsync(p, rot, Bs * 9 * 8, cudaMemcpyHostToDevice, h->stream)); dr = p; p += Bs * 9;
-    CK(cudaMemcpyAsync(p, foot, Bs * 12 * 8, cudaMemcpyHostToDevice, h->stream)); dfo = p; p += Bs * 12;
-    df = p; p += Bs * 12;
-    uint32_t* pc = (uint32_t*)p;
-    CK(cudaMemcpyAsync(pc, contact, Bs * 4, cudaMemcpyHostToDevice, h->stream)); dc = pc;
-    ds = (int32_t*)(pc + Bs);
-  }
+  if ((rc = st.begin())) return rc;
+  if ((rc = ensure_lists(h, (4 * (size_t)B + 8) * sizeof(int)))) return rc;
   {
     int nl = 0;
-    cudaError_t e = grf_qp_launch(h->sm_count, B, da, drz, dr, dfo, dc, df, ds, h->d_lists, h->stream, &nl);
+    cudaError_t e = grf_qp_launch(h->sm_count, B, root_acc, rot_z, rot, foot, contact, f_body, status, h->d_lists, h->stream, &nl);
     if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("grf_qp kernels: ") + cudaGetErrorString(e));
     h->launches += nl;
   }
-  if (!dev) {
-    CK(cudaMemcpyAsync(f_body, df, Bs * 12 * 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(status, ds, Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return A1MPC_OK;
+  return st.finish();
 }
 
 int a1mpc_joint_torques_batch(a1mpc_handle* h, int B, const double* f_grf, const double* f_kin, const double* jac, const uint32_t* contact,
@@ -717,35 +616,19 @@ int a1mpc_joint_torques_batch(a1mpc_handle* h, int B, const double* f_grf, const
   if (!h || !f_grf || !f_kin || !jac || !contact || !km_foot || !torques_gravity || !tau) return fail(A1MPC_EINVAL, "null argument");
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
   CK(cudaSetDevice(h->device));
-  const bool dev = is_device_ptr(f_grf);
-  if (mixed_sides(dev, {f_kin, jac, contact, tau})) return fail(A1MPC_EINVAL, "batch arrays must be all-host or all-device (km_foot, torques_gravity: always host)");
-  if (is_device_ptr(km_foot) || is_device_ptr(torques_gravity)) return fail(A1MPC_EINVAL, "km_foot and torques_gravity are host arrays (batch-uniform parameters)");
-  const size_t Bs = (size_t)B;
+  Stage st(h, B);
+  st.in(f_grf, 12); st.in(f_kin, 12); st.in(jac, 36); st.in(contact, 1);
+  st.inout(tau, 12);
+  st.host_param(km_foot, "km_foot"); st.host_param(torques_gravity, "torques_gravity");
+  int rc;
+  if ((rc = st.begin())) return rc;
   TorqueParams P;
   for (int i = 0; i < 3; ++i) P.km[i] = km_foot[i];
   for (int i = 0; i < 12; ++i) P.tg[i] = torques_gravity[i];
-  const double *dg = f_grf, *dk = f_kin, *dj = jac;
-  const uint32_t* dc = contact;
-  double* dt = tau;
-  int rc;
-  if (!dev) {
-    if ((rc = ensure_side(h, Bs * (12 + 12 + 36 + 12) * 8 + Bs * 4))) return rc;
-    double* p = (double*)h->d_side;
-    CK(cudaMemcpyAsync(p, f_grf, Bs * 12 * 8, cudaMemcpyHostToDevice, h->stream)); dg = p; p += Bs * 12;
-    CK(cudaMemcpyAsync(p, f_kin, Bs * 12 * 8, cudaMemcpyHostToDevice, h->stream)); dk = p; p += Bs * 12;
-    CK(cudaMemcpyAsync(p, jac, Bs * 36 * 8, cudaMemcpyHostToDevice, h->stream)); dj = p; p += Bs * 36;
-    CK(cudaMemcpyAsync(p, tau, Bs * 12 * 8, cudaMemcpyHostToDevice, h->stream)); dt = p; p += Bs * 12;
-    uint32_t* pc = (uint32_t*)p;
-    CK(cudaMemcpyAsync(pc, contact, Bs * 4, cudaMemcpyHostToDevice, h->stream)); dc = pc;
-  }
-  joint_torques_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, dg, dk, dj, dc, P, dt);
+  joint_torques_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, f_grf, f_kin, jac, contact, P, tau);
   h->launches++;
   CK(cudaGetLastError());
-  if (!dev) {
-    CK(cudaMemcpyAsync(tau, dt, Bs * 12 * 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return A1MPC_OK;
+  return st.finish();
 }
 
 int a1mpc_update_plan_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, double* gait_counter, const double* gait_counter_speed,
@@ -761,93 +644,24 @@ int a1mpc_update_plan_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp,
   G.cpg = gp->counter_per_gait; G.cps = gp->counter_per_swing; G.cdt = gp->control_dt; G.dxl = gp->foot_delta_x_limit; G.dyl = gp->foot_delta_y_limit;
   for (int i = 0; i < 12; ++i) G.dfp[i] = gp->default_foot_pos[i];
   G.N = gp->horizon;
-  const bool dev = is_device_ptr(gait_counter);
-  const size_t Bs = (size_t)B;
+  Stage st(h, B);
+  st.inout(gait_counter, 4); st.in(gait_counter_speed, 4); st.in(movement_mode, 1);
+  if (want_t) {   // the kernel reads the foothold inputs only for the foothold outputs
+    st.in(lin_vel, 3); st.in(lin_vel_d, 3); st.in(rot_z, 9); st.in(rot, 9); st.in(root_pos, 3);
+  } else {
+    for (const void* p : {lin_vel, lin_vel_d, rot_z, rot, root_pos}) st.unused(p);
+  }
+  st.out(plan_contacts, 1); st.out(contact_sched, G.N); st.out(t_rel, 12); st.out(t_abs, 12); st.out(t_world, 12);
   int rc;
-  if (dev) {
-    update_plan_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, G, gait_counter, gait_counter_speed, movement_mode, lin_vel, lin_vel_d, rot_z, rot, root_pos,
-                                                                plan_contacts, contact_sched, t_rel, t_abs, t_world);
-    h->launches++;
-    CK(cudaGetLastError());
-    return A1MPC_OK;
-  }
-  // host pointers: stage everything in one scratch allocation
-  const size_t nd = Bs * (4 + 4 + 3 + 3 + 9 + 9 + 3 + 36), nu = Bs * (1 + 1 + (size_t)G.N);
-  if ((rc = ensure_side(h, nd * 8 + nu * 4))) return rc;
-  double* p = (double*)h->d_side;
-  double* d_gc = p; p += 4 * Bs;
-  double* d_gcs = p; p += 4 * Bs;
-  double* d_lv = p; p += 3 * Bs;
-  double* d_lvd = p; p += 3 * Bs;
-  double* d_rz = p; p += 9 * Bs;
-  double* d_r = p; p += 9 * Bs;
-  double* d_pos = p; p += 3 * Bs;
-  double* d_trel = p; p += 12 * Bs;
-  double* d_tabs = p; p += 12 * Bs;
-  double* d_tw = p; p += 12 * Bs;
-  uint32_t* u = (uint32_t*)p;
-  uint32_t* d_mode = u; u += Bs;
-  uint32_t* d_plan = u; u += Bs;
-  uint32_t* d_sched = u;
-  CK(cudaMemcpyAsync(d_gc, gait_counter, 4 * Bs * 8, cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(d_gcs, gait_counter_speed, 4 * Bs * 8, cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(d_mode, movement_mode, Bs * 4, cudaMemcpyHostToDevice, h->stream));
-  if (want_t) {
-    CK(cudaMemcpyAsync(d_lv, lin_vel, 3 * Bs * 8, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(d_lvd, lin_vel_d, 3 * Bs * 8, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(d_rz, rot_z, 9 * Bs * 8, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(d_r, rot, 9 * Bs * 8, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(d_pos, root_pos, 3 * Bs * 8, cudaMemcpyHostToDevice, h->stream));
-  }
-  update_plan_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, G, d_gc, d_gcs, d_mode, d_lv, d_lvd, d_rz, d_r, d_pos, d_plan, contact_sched ? d_sched : nullptr,
-                                                              t_rel ? d_trel : nullptr, t_abs ? d_tabs : nullptr, t_world ? d_tw : nullptr);
+  if ((rc = st.begin())) return rc;
+  update_plan_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, G, gait_counter, gait_counter_speed, movement_mode, lin_vel, lin_vel_d, rot_z, rot,
+                                                              root_pos, plan_contacts, contact_sched, t_rel, t_abs, t_world);
   h->launches++;
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(gait_counter, d_gc, 4 * Bs * 8, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(plan_contacts, d_plan, Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (contact_sched) CK(cudaMemcpyAsync(contact_sched, d_sched, (size_t)G.N * Bs * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (t_rel) CK(cudaMemcpyAsync(t_rel, d_trel, 12 * Bs * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (t_abs) CK(cudaMemcpyAsync(t_abs, d_tabs, 12 * Bs * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (t_world) CK(cudaMemcpyAsync(t_world, d_tw, 12 * Bs * 8, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return A1MPC_OK;
+  return st.finish();
 }
 
 // ---- upstream producers of the path's inputs (SURVEY 8f.4) ---------------------------------------------------
-}  // extern "C"
-namespace {
-// host-pointer mode of the side entry points: inputs are staged into h->d_side, outputs copied back after the kernel
-struct Stage {
-  a1mpc_handle* h;
-  bool host;
-  char* cur = nullptr;
-  struct Out { void* host; const void* dev; size_t bytes; };
-  std::vector<Out> outs;
-  static size_t pad(size_t b) { return (b + 255) & ~(size_t)255; }
-  template <class T>
-  int in(const T*& p, size_t bytes) {
-    if (!host || !p) return A1MPC_OK;
-    CK(cudaMemcpyAsync(cur, p, bytes, cudaMemcpyHostToDevice, h->stream));
-    p = reinterpret_cast<const T*>(cur);
-    cur += pad(bytes);
-    return A1MPC_OK;
-  }
-  template <class T>
-  void out(T*& p, size_t bytes) {
-    if (!host || !p) return;
-    outs.push_back({p, cur, bytes});
-    p = reinterpret_cast<T*>(cur);
-    cur += pad(bytes);
-  }
-  int finish() {
-    if (!host) return A1MPC_OK;
-    for (const Out& o : outs) CK(cudaMemcpyAsync(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    return A1MPC_OK;
-  }
-};
-}  // namespace
-extern "C" {
 
 int a1mpc_leg_kinematics_batch(a1mpc_handle* h, int B, const double* joint_pos, const double* joint_vel, const double* rot,
                                const double* rho_opt, const double* rho_fix, double* foot_pos_rel, double* jac, double* foot_vel_rel,
@@ -857,21 +671,15 @@ int a1mpc_leg_kinematics_batch(a1mpc_handle* h, int B, const double* joint_pos, 
   if ((foot_vel_rel || foot_vel_abs) && !joint_vel) return fail(A1MPC_EINVAL, "foot velocities need joint_vel");
   if ((foot_pos_abs || foot_vel_abs) && !rot) return fail(A1MPC_EINVAL, "body-aligned outputs need rot");
   CK(cudaSetDevice(h->device));
-  const size_t Bs = (size_t)B;
+  Stage st(h, B);
+  st.in(joint_pos, 12); st.in(joint_vel, 12); st.in(rot, 9);
+  st.out(foot_pos_rel, 12); st.out(jac, 36); st.out(foot_vel_rel, 12); st.out(foot_pos_abs, 12); st.out(foot_vel_abs, 12);
+  st.host_param(rho_opt, "rho_opt"); st.host_param(rho_fix, "rho_fix");
+  int rc;
+  if ((rc = st.begin())) return rc;
   LegParams P;
   for (int i = 0; i < 12; ++i) P.rho_opt[i] = rho_opt[i];
   for (int i = 0; i < 20; ++i) P.rho_fix[i] = rho_fix[i];
-  Stage st{h, !is_device_ptr(joint_pos)};
-  int rc;
-  if (st.host) {
-    if ((rc = ensure_side(h, 8 * Stage::pad(36 * Bs * 8)))) return rc;
-    st.cur = (char*)h->d_side;
-  }
-  if ((rc = st.in(joint_pos, 12 * Bs * 8))) return rc;
-  if ((rc = st.in(joint_vel, 12 * Bs * 8))) return rc;
-  if ((rc = st.in(rot, 9 * Bs * 8))) return rc;
-  st.out(foot_pos_rel, 12 * Bs * 8); st.out(jac, 36 * Bs * 8); st.out(foot_vel_rel, 12 * Bs * 8);
-  st.out(foot_pos_abs, 12 * Bs * 8); st.out(foot_vel_abs, 12 * Bs * 8);
   leg_kinematics_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, joint_pos, joint_vel, rot, P, foot_pos_rel, jac, foot_vel_rel, foot_pos_abs, foot_vel_abs);
   h->launches++;
   CK(cudaGetLastError());
@@ -885,15 +693,10 @@ int a1mpc_ekf_init_batch(a1mpc_handle* h, int B, void* ekf_state, const double* 
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
   CK(cudaSetDevice(h->device));
   if (!is_device_ptr(ekf_state)) return fail(A1MPC_EINVAL, "ekf_state must be device memory (a1mpc_device_alloc)");
-  const size_t Bs = (size_t)B;
-  Stage st{h, !is_device_ptr(foot_pos_rel)};
+  Stage st(h, B);
+  st.in(foot_pos_rel, 12); st.in(rot, 9);
   int rc;
-  if (st.host) {
-    if ((rc = ensure_side(h, 2 * Stage::pad(12 * Bs * 8)))) return rc;
-    st.cur = (char*)h->d_side;
-  }
-  if ((rc = st.in(foot_pos_rel, 12 * Bs * 8))) return rc;
-  if ((rc = st.in(rot, 9 * Bs * 8))) return rc;
+  if ((rc = st.begin())) return rc;
   ekf_init_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, static_cast<double*>(ekf_state), foot_pos_rel, rot);
   h->launches++;
   CK(cudaGetLastError());
@@ -916,21 +719,12 @@ int a1mpc_ekf_update_batch(a1mpc_handle* h, int B, void* ekf_state, double dt, i
     CK(cudaFuncSetAttribute(ekf_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set[h->device] = true;
   }
-  const size_t Bs = (size_t)B;
-  Stage st{h, !is_device_ptr(imu_acc)};
+  Stage st(h, B);
+  st.in(movement_mode, 1); st.in(imu_acc, 3); st.in(imu_ang_vel, 3); st.in(rot, 9); st.in(foot_pos_rel, 12); st.in(foot_vel_rel, 12);
+  st.in(foot_force, 4);
+  st.out(root_pos, 3); st.out(root_lin_vel, 3); st.out(estimated_contacts, 1); st.out(status, 1);
   int rc;
-  if (st.host) {
-    if ((rc = ensure_side(h, 12 * Stage::pad(12 * Bs * 8)))) return rc;
-    st.cur = (char*)h->d_side;
-  }
-  if ((rc = st.in(movement_mode, Bs * 4))) return rc;
-  if ((rc = st.in(imu_acc, 3 * Bs * 8))) return rc;
-  if ((rc = st.in(imu_ang_vel, 3 * Bs * 8))) return rc;
-  if ((rc = st.in(rot, 9 * Bs * 8))) return rc;
-  if ((rc = st.in(foot_pos_rel, 12 * Bs * 8))) return rc;
-  if ((rc = st.in(foot_vel_rel, 12 * Bs * 8))) return rc;
-  if ((rc = st.in(foot_force, 4 * Bs * 8))) return rc;
-  st.out(root_pos, 3 * Bs * 8); st.out(root_lin_vel, 3 * Bs * 8); st.out(estimated_contacts, Bs * 4); st.out(status, Bs * 4);
+  if ((rc = st.begin())) return rc;
   EkfParams P{dt, assume_flat_ground ? 1 : 0};
   int grid = (B + EKF_WPC - 1) / EKF_WPC;
   if (grid > h->sm_count * 2) grid = h->sm_count * 2;
@@ -966,28 +760,16 @@ int a1mpc_swing_legs_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, 
   if (!(dt > 0.0) || !(gp->counter_per_swing > 0.0)) return fail(A1MPC_EINVAL, "dt and counter_per_swing must be positive");
   CK(cudaSetDevice(h->device));
   if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
-  if (is_device_ptr(kp_foot) || is_device_ptr(kd_foot)) return fail(A1MPC_EINVAL, "kp_foot and kd_foot are host arrays (batch-uniform parameters)");
-  const bool dev = is_device_ptr(gait_counter);
-  if (mixed_sides(dev, {plan_contacts, rot_z, foot_pos_abs, foot_pos_target_rel, foot_force, f_kin, contacts, foot_pos_cur, foot_pos_recent_contact}))
-    return fail(A1MPC_EINVAL, "batch arrays must be all-host or all-device (kp_foot, kd_foot: always host)");
+  Stage st(h, B);
+  st.in(gait_counter, 4); st.in(plan_contacts, 1); st.in(rot_z, 9); st.in(foot_pos_abs, 12); st.in(foot_pos_target_rel, 12); st.in(foot_force, 4);
+  st.out(f_kin, 12); st.out(contacts, 1); st.out(foot_pos_cur, 12); st.out(foot_pos_recent_contact, 12);
+  st.host_param(kp_foot, "kp_foot"); st.host_param(kd_foot, "kd_foot");
+  int rc;
+  if ((rc = st.begin())) return rc;
   SwingParams P;
   P.cps = gp->counter_per_swing;
   P.dt = dt;
   for (int i = 0; i < 12; ++i) { P.kp[i] = kp_foot[i]; P.kd[i] = kd_foot[i]; }
-  const size_t Bs = (size_t)B;
-  Stage st{h, !dev};
-  int rc;
-  if (st.host) {
-    if ((rc = ensure_side(h, 11 * Stage::pad(12 * Bs * 8)))) return rc;
-    st.cur = (char*)h->d_side;
-  }
-  if ((rc = st.in(gait_counter, 4 * Bs * 8))) return rc;
-  if ((rc = st.in(plan_contacts, Bs * 4))) return rc;
-  if ((rc = st.in(rot_z, 9 * Bs * 8))) return rc;
-  if ((rc = st.in(foot_pos_abs, 12 * Bs * 8))) return rc;
-  if ((rc = st.in(foot_pos_target_rel, 12 * Bs * 8))) return rc;
-  if ((rc = st.in(foot_force, 4 * Bs * 8))) return rc;
-  st.out(f_kin, 12 * Bs * 8); st.out(contacts, Bs * 4); st.out(foot_pos_cur, 12 * Bs * 8); st.out(foot_pos_recent_contact, 12 * Bs * 8);
   swing_legs_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, P, static_cast<double*>(swing_state), gait_counter, plan_contacts, rot_z, foot_pos_abs,
                                                             foot_pos_target_rel, foot_force, f_kin, contacts, foot_pos_cur, foot_pos_recent_contact);
   h->launches++;
@@ -1002,22 +784,16 @@ int a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use
   if (ref && ref_ld < (size_t)B) return fail(A1MPC_EINVAL, "ref_ld must be >= B");
   CK(cudaSetDevice(h->device));
   if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
-  const bool dev = is_device_ptr(root_pos);
-  if (mixed_sides(dev, {ref, terrain_pitch})) return fail(A1MPC_EINVAL, "batch arrays must be all-host or all-device");
-  const size_t Bs = (size_t)B;
   // only row 1 of ref is written: on the host side it is staged as a dense row (ld 0 from the kernel's point of view)
   double* row = use_terrain_adapt ? ref + ref_ld : nullptr;
-  size_t kld = ref_ld;
-  Stage st{h, !dev};
+  Stage st(h, B);
+  st.in(root_pos, 3);
+  st.out(row, 1); st.out(terrain_pitch, 1);
+  if (!use_terrain_adapt) st.unused(ref);
   int rc;
-  if (st.host) {
-    if ((rc = ensure_side(h, 3 * Stage::pad(3 * Bs * 8)))) return rc;
-    st.cur = (char*)h->d_side;
-    kld = 0;
-  }
-  if ((rc = st.in(root_pos, 3 * Bs * 8))) return rc;
-  st.out(row, Bs * 8); st.out(terrain_pitch, Bs * 8);
-  double* kref = st.host ? row : ref;
+  if ((rc = st.begin())) return rc;
+  double* kref = st.host() ? row : ref;
+  const size_t kld = st.host() ? 0 : ref_ld;
   terrain_pitch_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, static_cast<double*>(swing_state), use_terrain_adapt ? 1 : 0, root_pos, kref, kld,
                                                                terrain_pitch);
   h->launches++;
