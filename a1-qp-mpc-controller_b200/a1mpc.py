@@ -18,7 +18,7 @@ STATUS_OPTIMAL, STATUS_IPM_ONLY, STATUS_MAXITER, STATUS_NUMERICAL, STATUS_NO_CON
 EXPORTS = [
     "a1mpc_default_config", "a1mpc_create", "a1mpc_destroy", "a1mpc_last_error", "a1mpc_device_count",
     "a1mpc_solve_batch", "a1mpc_warm_bytes", "a1mpc_warm_reset", "a1mpc_solve_batch_warm", "a1mpc_solve_batch_ext", "a1mpc_solve_batch_ext_warm", "a1mpc_build_qp_batch", "a1mpc_qp_mats_batch", "a1mpc_solve_dense_batch",
-    "a1mpc_grf_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
+    "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
     "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
@@ -115,6 +115,7 @@ def lib():
         l.a1mpc_qp_rollout_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 8
         l.a1mpc_solve_dense_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
         l.a1mpc_grf_qp_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
+        l.a1mpc_stance_qp_batch.argtypes = [C.c_void_p, C.c_int, C.c_size_t] + [C.c_void_p] * 13
         l.a1mpc_joint_torques_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
         l.a1mpc_update_plan_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams)] + [C.c_void_p] * 13
         l.a1mpc_swing_bytes.restype = C.c_size_t
@@ -329,6 +330,21 @@ class Engine:
         f = np.zeros((B, 12)); status = np.zeros(B, dtype=np.int32)
         _check(lib().a1mpc_grf_qp_batch(self.h, B, _p(arrs[0]), _p(arrs[1]), _p(arrs[2]), _p(arrs[3]), _p(contact), _p(f), _p(status)))
         return f, status
+
+    def stance_qp(self, x0, rot, rot_z, foot, contact, des, kp_linear, kd_linear, kp_angular, kd_angular, want_acc=False):
+        """a1mpc_stance_qp_batch (compute_grf's QP branch from the controller state), batch-major host arrays: x0 [12,B], rot / rot_z [9,B],
+        foot [12,B], contact [B], des [12,B] (root_euler_d, root_pos_d, root_lin_vel_d, root_ang_vel_d), kp_linear [3,B]; kd_linear,
+        kp_angular, kd_angular [3] -> f_body [12,B], status [B] (, root_acc [6,B] when want_acc)"""
+        a = [np.ascontiguousarray(v, dtype=np.float64) for v in (x0, rot, rot_z, foot)]
+        contact = np.ascontiguousarray(contact, dtype=np.uint32)
+        d, kpl = np.ascontiguousarray(des, dtype=np.float64), np.ascontiguousarray(kp_linear, dtype=np.float64)
+        g = [np.ascontiguousarray(v, dtype=np.float64) for v in (kd_linear, kp_angular, kd_angular)]
+        B = contact.shape[0]
+        f = np.zeros((12, B)); status = np.zeros(B, dtype=np.int32)
+        acc = np.zeros((6, B)) if want_acc else None
+        _check(lib().a1mpc_stance_qp_batch(self.h, B, B, *[_p(v) for v in a], _p(contact), _p(d), _p(kpl), *[_p(v) for v in g], _p(f), _p(status),
+                                           _p(acc)))
+        return (f, status, acc) if want_acc else (f, status)
 
     def joint_torques(self, f_grf, f_kin, jac, contact, km_foot, torques_gravity, tau_prev=None):
         """batch-major SoA [12,B], [12,B], [36,B], [B] -> tau [12,B]"""

@@ -611,6 +611,35 @@ int a1mpc_grf_qp_batch(a1mpc_handle* h, int B, const double* root_acc, const dou
   return st.finish();
 }
 
+int a1mpc_stance_qp_batch(a1mpc_handle* h, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
+                          const uint32_t* contact, const double* des, const double* kp_linear, const double* kd_linear, const double* kp_angular,
+                          const double* kd_angular, double* f_body, int32_t* status, double* root_acc) {
+  if (!h || !x0 || !rot || !rot_z || !foot || !contact || !des || !kp_linear || !kd_linear || !kp_angular || !kd_angular || !f_body || !status)
+    return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (ld < (size_t)B) return fail(A1MPC_EINVAL, "ld < B");
+  CK(cudaSetDevice(h->device));
+  Stage st(h, B);
+  st.in(x0, 12, 8, ld); st.in(rot, 9, 8, ld); st.in(rot_z, 9, 8, ld); st.in(foot, 12, 8, ld); st.in(contact, 1);
+  st.in(des, 12, 8, ld); st.in(kp_linear, 3, 8, ld);
+  st.out(f_body, 12, 8, ld); st.out(status, 1); st.out(root_acc, 6, 8, ld);
+  st.host_param(kd_linear, "kd_linear"); st.host_param(kp_angular, "kp_angular"); st.host_param(kd_angular, "kd_angular");
+  int rc;
+  if ((rc = st.begin())) return rc;
+  const size_t kld = st.host() ? (size_t)B : ld;
+  if ((rc = ensure_lists(h, stance_scratch_bytes(B)))) return rc;
+  double gains[9];
+  for (int i = 0; i < 3; ++i) { gains[i] = kd_linear[i]; gains[3 + i] = kp_angular[i]; gains[6 + i] = kd_angular[i]; }
+  {
+    int nl = 0;
+    cudaError_t e = stance_qp_launch(h->sm_count, B, kld, x0, rot, rot_z, foot, contact, des, kp_linear, gains, h->cfg.mass, f_body, status,
+                                     root_acc, h->d_lists, h->stream, &nl);
+    if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("stance_qp kernels: ") + cudaGetErrorString(e));
+    h->launches += nl;
+  }
+  return st.finish();
+}
+
 int a1mpc_joint_torques_batch(a1mpc_handle* h, int B, const double* f_grf, const double* f_kin, const double* jac, const uint32_t* contact,
                               const double* km_foot, const double* torques_gravity, double* tau) {
   if (!h || !f_grf || !f_kin || !jac || !contact || !km_foot || !torques_gravity || !tau) return fail(A1MPC_EINVAL, "null argument");
