@@ -84,6 +84,9 @@ struct a1mpc_handle {
     bool opened[MAX_PEERS] = {false};
     unsigned long long step = 0;
   } peer;
+#if A1MPC_TIMELINE
+  unsigned long long* tl = nullptr;   // measurement build: timeline records of the class kernels (a1mpc_timeline_attach)
+#endif
 };
 
 namespace {
@@ -254,6 +257,9 @@ int peer_signal(a1mpc_handle* h, int B) {
 int enqueue_solve(a1mpc_handle* h, int B, const DevInputs& din, const DevOutputs& dout_in, uint32_t* warm = nullptr, int shift = 0) {
   DevOutputs dout = dout_in;
   attach_peers(h, B, dout);
+#if A1MPC_TIMELINE
+  dout.tl = h->tl;
+#endif
   CK(cudaMemsetAsync(h->d_count, 0, 16 * sizeof(int), h->stream));
   pack_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(din, B, h->d_rec, (int)h->cap, h->d_count, dout, h->cfg.horizon);
   h->launches++;
@@ -294,6 +300,9 @@ int enqueue_solve_ext(a1mpc_handle* h, int B, const DevInputs& di, const uint32_
   }
   DevOutputs dout = dout_in;
   attach_peers(h, -1, dout);   // the fused collect is wired to a1mpc_solve_batch / _warm only
+#if A1MPC_TIMELINE
+  dout.tl = h->tl;
+#endif
   CK(cudaMemsetAsync(h->d_count, 0, 16 * sizeof(int), h->stream));
   if (warm) {   // robots without any contact are answered by the pack kernel and store no guess
     warm_forget_no_contact_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, B, warm, N);
@@ -909,6 +918,16 @@ int a1mpc_event_elapsed_ms(a1mpc_handle* h, void* start, void* stop, float* ms) 
   return A1MPC_OK;
 }
 int64_t a1mpc_launch_count(const a1mpc_handle* h) { return h ? h->launches : 0; }
+
+#if A1MPC_TIMELINE
+// measurement build only (tools/timeline.py): device buffer of a1mpc::TL_CLASSES * (TL_CTAS + TL_QPS) * 4 u64 that the class kernels
+// of every later solve write their CTA and QP records into (layout at tl_cta in a1mpc_device.cuh); NULL detaches it
+int a1mpc_timeline_attach(a1mpc_handle* h, void* buf) {
+  if (!h) return fail(A1MPC_EINVAL, "null handle");
+  h->tl = static_cast<unsigned long long*>(buf);
+  return A1MPC_OK;
+}
+#endif
 
 int a1mpc_measure_fp64_peak(a1mpc_handle* h, double* tflops) {
   if (!h || !tflops) return fail(A1MPC_EINVAL, "null argument");
