@@ -7,11 +7,21 @@ namespace a1mpc {
 // -------------------------------------------------------------------------------------------
 // pack kernel: SoA batch -> per-class records.  Thread-per-QP, every load is a coalesced 64-bit
 // batch-major access (32 consecutive QPs per warp instruction).
+// All 42 inputs and the contact mask are loaded before the slot is claimed and before the first store, so that they are in
+// flight together: loaded and stored field by field, each load waits for the store before it (the compiler cannot rule out
+// that a record store overwrites an input) and a thread runs a chain of 42 HBM round trips.
 // -------------------------------------------------------------------------------------------
-__global__ void pack_kernel(DevInputs in, int B, double* __restrict__ rec, int cap, int* __restrict__ count,
-                            DevOutputs out, int horizon) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+__device__ __forceinline__ void pack_one(const DevInputs& in, int b, double* __restrict__ rec, int cap, int* __restrict__ count,
+                                         const DevOutputs& out, int horizon) {
+  double v[REC_DOUBLES];
+#pragma unroll
+  for (int k = 0; k < 12; ++k) v[k] = ld_in(in.x0, (size_t)k * in.ld + b, in.f32);
+#pragma unroll
+  for (int k = 0; k < 9; ++k) v[12 + k] = ld_in(in.rot, (size_t)k * in.ld + b, in.f32);
+#pragma unroll
+  for (int k = 0; k < 12; ++k) v[21 + k] = ld_in(in.foot, (size_t)k * in.ld + b, in.f32);
+#pragma unroll
+  for (int k = 0; k < 9; ++k) v[33 + k] = ld_in(in.ref, (size_t)k * in.ld + b, in.f32);
   const uint32_t mask = in.contact[b] & 15u;
   const int ns = __popc(mask);
   if (ns == 0) {  // every foot is pinned to zero by fz in [0,0] (ConvexMpc.cpp:233,238)
@@ -23,17 +33,23 @@ __global__ void pack_kernel(DevInputs in, int B, double* __restrict__ rec, int c
     return;
   }
   const int slot = atomicAdd(&count[ns], 1);
-  double* r = rec + ((size_t)(ns - 1) * cap + slot) * REC_DOUBLES;
+  v[42] = __hiloint2double((int)mask, b);
+  v[43] = 0.0;
+  double2* r = reinterpret_cast<double2*>(rec + ((size_t)(ns - 1) * cap + slot) * REC_DOUBLES);   // 352-byte records: 16-byte aligned
 #pragma unroll
-  for (int k = 0; k < 12; ++k) r[k] = ld_in(in.x0, (size_t)k * in.ld + b, in.f32);
-#pragma unroll
-  for (int k = 0; k < 9; ++k) r[12 + k] = ld_in(in.rot, (size_t)k * in.ld + b, in.f32);
-#pragma unroll
-  for (int k = 0; k < 12; ++k) r[21 + k] = ld_in(in.foot, (size_t)k * in.ld + b, in.f32);
-#pragma unroll
-  for (int k = 0; k < 9; ++k) r[33 + k] = ld_in(in.ref, (size_t)k * in.ld + b, in.f32);
-  r[42] = __hiloint2double((int)mask, b);
-  r[43] = 0.0;
+  for (int k = 0; k < REC_DOUBLES / 2; ++k) r[k] = make_double2(v[2 * k], v[2 * k + 1]);
+}
+
+__global__ void pack_kernel(DevInputs in, int B, double* __restrict__ rec, int cap, int* __restrict__ count,
+                            DevOutputs out, int horizon) {
+#if A1MPC_TIMELINE
+  tl_enter(out, TL_PACK);
+#endif
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) pack_one(in, b, rec, cap, count, out, horizon);
+#if A1MPC_TIMELINE
+  tl_leave(out, TL_PACK);
+#endif
 }
 
 // pack kernel of the extended path: one 464-byte record per QP (base record + per-step contact masks + unit normals)
