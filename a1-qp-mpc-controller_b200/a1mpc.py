@@ -19,7 +19,9 @@ EXPORTS = [
     "a1mpc_default_config", "a1mpc_create", "a1mpc_destroy", "a1mpc_last_error", "a1mpc_device_count",
     "a1mpc_solve_batch", "a1mpc_warm_bytes", "a1mpc_warm_reset", "a1mpc_solve_batch_warm", "a1mpc_solve_batch_ext", "a1mpc_solve_batch_ext_warm", "a1mpc_build_qp_batch", "a1mpc_qp_mats_batch", "a1mpc_solve_dense_batch",
     "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
-    "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
+    "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch",
+    "a1mpc_imu_bytes", "a1mpc_imu_init_batch", "a1mpc_orientation_batch", "a1mpc_command_bytes", "a1mpc_command_init_batch", "a1mpc_command_batch",
+    "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
     "a1mpc_flush_l2", "a1mpc_profile_begin", "a1mpc_profile_end", "a1mpc_nccl_unique_id", "a1mpc_nccl_init", "a1mpc_allgather_forces",
@@ -53,6 +55,26 @@ def default_gait_params(horizon=10):
     g.default_foot_pos[:] = [0.17, 0.17, -0.17, -0.17, 0.15, -0.15, 0.15, -0.15, -0.35, -0.35, -0.35, -0.35]
     g.foot_delta_x_limit, g.foot_delta_y_limit, g.horizon = 0.1, 0.1, horizon
     return g
+
+
+VARIANT_GAZEBO, VARIANT_HARDWARE, VARIANT_ISAAC = 0, 1, 2
+
+
+class CommandParams(C.Structure):
+    _fields_ = [("variant", C.c_int), ("body_height", C.c_double), ("body_height_min", C.c_double), ("body_height_max", C.c_double),
+                ("kp_linear", C.c_double * 3), ("kp_linear_lock", C.c_double * 2)]
+
+
+def default_command_params(variant=VARIANT_GAZEBO):
+    """the adapter's initial joy_cmd_body_height (GazeboA1ROS.h:130, HardwareA1ROS.h:107, IsaacA1ROS.h:80), JOY_CMD_BODY_HEIGHT_MIN / _MAX
+    (A1Params.h:16-17) and the ROS-parameter defaults of kp_linear and its lock gains (A1CtrlStates.h:270-301)"""
+    c = CommandParams()
+    c.variant = variant
+    c.body_height = {VARIANT_GAZEBO: 0.3, VARIANT_HARDWARE: 0.12, VARIANT_ISAAC: 0.32}.get(variant, 0.3)
+    c.body_height_min, c.body_height_max = 0.1, 0.32
+    c.kp_linear[:] = [120.0, 120.0, 500.0]
+    c.kp_linear_lock[:] = [120.0, 120.0]
+    return c
 
 
 class InputsExt(C.Structure):
@@ -123,6 +145,14 @@ def lib():
         l.a1mpc_swing_init_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         l.a1mpc_swing_legs_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_double] + [C.c_void_p] * 10
         l.a1mpc_terrain_pitch_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        for name in ("a1mpc_imu_bytes", "a1mpc_command_bytes"):
+            getattr(l, name).restype = C.c_size_t
+            getattr(l, name).argtypes = [C.c_int]
+        l.a1mpc_imu_init_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        l.a1mpc_orientation_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7 + [C.c_size_t, C.c_void_p, C.c_void_p]
+        l.a1mpc_command_init_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(CommandParams), C.c_void_p, C.c_size_t]
+        l.a1mpc_command_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
         l.a1mpc_gen_states.argtypes = [C.c_int, C.c_uint64, C.c_int] + [C.c_void_p] * 5
         l.a1mpc_measure_fp64_peak.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         l.a1mpc_profile_begin.argtypes = [C.c_void_p, C.c_int]
@@ -424,6 +454,53 @@ class Engine:
         _check(lib().a1mpc_terrain_pitch_batch(self.h, B, swing, int(use_terrain_adapt), _p(pos), _p(ref), ref.shape[1] if ref is not None else B,
                                                _p(pitch)))
         return pitch
+
+    def imu_alloc(self, B):
+        """device-resident IMU filter state of B robots (a1mpc_imu_bytes), initialised by a1mpc_imu_init_batch; bound to this B"""
+        p = self.dalloc(lib().a1mpc_imu_bytes(B))
+        self.imu_init(p, B)
+        return p
+
+    def imu_init(self, imu, B):
+        """a1mpc_imu_init_batch: six empty MovingWindowFilter(5)"""
+        _check(lib().a1mpc_imu_init_batch(self.h, B, imu))
+
+    def orientation(self, quat, gyro, acc=None, imu=None):
+        """a1mpc_orientation_batch, host arrays: quat [4,B] (w, x, y, z), gyro / acc [3,B]; imu = the filter state or None (unfiltered) ->
+        dict rot [9,B], rot_z [9,B], euler [3,B], ang_vel [3,B] (x0 rows 0-2 and 6-8), imu_acc [3,B] (None without acc), imu_ang_vel [3,B]"""
+        q, g = [np.ascontiguousarray(v, dtype=np.float64) for v in (quat, gyro)]
+        a = np.ascontiguousarray(acc, dtype=np.float64) if acc is not None else None
+        B = q.shape[1]
+        x0 = np.zeros((12, B)); rot = np.zeros((9, B)); rz = np.zeros((9, B)); ia = np.zeros((3, B)) if a is not None else None; ig = np.zeros((3, B))
+        _check(lib().a1mpc_orientation_batch(self.h, B, _p(q), _p(g), _p(a), imu, _p(rot), _p(rz), _p(x0), B, _p(ia), _p(ig)))
+        return dict(rot=rot, rot_z=rz, euler=x0[0:3].copy(), ang_vel=x0[6:9].copy(), imu_acc=ia, imu_ang_vel=ig)
+
+    def command_alloc(self, B, params=None, ref=None):
+        """device-resident command state of B robots (a1mpc_command_bytes), initialised by a1mpc_command_init_batch from params
+        (default_command_params()); ref [9,B] (host, written in place) gets the reset rows.  Bound to this B"""
+        p = self.dalloc(lib().a1mpc_command_bytes(B))
+        self.command_init(p, B, params, ref)
+        return p
+
+    def command_init(self, cmd_state, B, params=None, ref=None):
+        """a1mpc_command_init_batch"""
+        cp = params if params is not None else default_command_params()
+        if ref is not None and not (ref.dtype == np.float64 and ref.flags["C_CONTIGUOUS"]):
+            raise A1MpcError("ref must be a C-contiguous float64 array (written in place)")
+        _check(lib().a1mpc_command_init_batch(self.h, B, cmd_state, C.byref(cp), _p(ref), ref.shape[1] if ref is not None else B))
+
+    def command(self, cmd_state, dt, cmd, root_pos, ref=None):
+        """a1mpc_command_batch, host arrays: cmd [7,B] (velx, vely, velz, roll / pitch / yaw rate, toggle), root_pos [3,B]; ref [9,B]
+        (a1mpc_inputs.ref layout, in / out in place: row 1 is this tick's starting root_euler_d[1]) ->
+        movement_mode [B], kp_linear [3,B], des [12,B] (a1mpc_stance_qp_batch layout)"""
+        c, pos = [np.ascontiguousarray(v, dtype=np.float64) for v in (cmd, root_pos)]
+        B = c.shape[1]
+        if ref is not None and not (ref.dtype == np.float64 and ref.flags["C_CONTIGUOUS"]):
+            raise A1MpcError("ref must be a C-contiguous float64 array (written in place)")
+        mode = np.zeros(B, dtype=np.uint32); kp = np.zeros((3, B)); des = np.zeros((12, B))
+        _check(lib().a1mpc_command_batch(self.h, B, cmd_state, C.c_double(dt), _p(c), _p(pos), B, _p(mode), _p(kp), _p(ref),
+                                         ref.shape[1] if ref is not None else B, _p(des), B))
+        return mode, kp, des
 
     def update_plan(self, gp, gait_counter, gait_counter_speed, movement_mode, lin_vel, lin_vel_d, rot_z, rot, root_pos):
         """A1RobotControl::update_plan batched; returns new gait_counter [4,B], plan_contacts [B], contact_sched [N,B],

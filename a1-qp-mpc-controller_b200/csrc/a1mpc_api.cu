@@ -151,6 +151,7 @@ class Stage {
   template <class T> void out(T*& p, size_t rows, size_t esz = sizeof(T)) { add(p, OUT, rows, esz, B_); }
   template <class T> void out(T*& p, size_t rows, size_t esz, size_t ld) { add(p, OUT, rows, esz, ld); }
   template <class T> void inout(T*& p, size_t rows, size_t esz = sizeof(T)) { add(p, INOUT, rows, esz, B_); }
+  template <class T> void inout(T*& p, size_t rows, size_t esz, size_t ld) { add(p, INOUT, rows, esz, ld); }
   // a batch array this call does not read: its side is checked, nothing is copied
   void unused(const void* p) { arrays_.push_back({nullptr, nullptr, const_cast<void*>(p), 0, 0, 0, UNUSED, nullptr}); }
   // a batch-uniform parameter read by the call itself on the host
@@ -836,6 +837,82 @@ int a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use
                                                                terrain_pitch);
   h->launches++;
   CK(cudaGetLastError());
+  return st.finish();
+}
+
+// ---- orientation and command stages (the adapters' IMU / pose callbacks and main_update's front half) ------------------------
+size_t a1mpc_imu_bytes(int B) { return B > 0 ? (size_t)B * imu_state_doubles() * sizeof(double) : 0; }
+
+int a1mpc_imu_init_batch(a1mpc_handle* h, int B, void* imu_state) {
+  if (!h || !imu_state) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(imu_state)) return fail(A1MPC_EINVAL, "imu_state must be device memory (a1mpc_device_alloc)");
+  CK(imu_init_launch(B, static_cast<double*>(imu_state), h->stream));
+  h->launches++;
+  return A1MPC_OK;
+}
+
+int a1mpc_orientation_batch(a1mpc_handle* h, int B, const double* quat, const double* gyro, const double* acc, void* imu_state, double* rot,
+                            double* rot_z, double* x0, size_t ld, double* imu_acc, double* imu_ang_vel) {
+  if (!h || !quat || !gyro) return fail(A1MPC_EINVAL, "null argument");
+  if (imu_acc && !acc) return fail(A1MPC_EINVAL, "imu_acc needs acc");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (ld < (size_t)B) return fail(A1MPC_EINVAL, "ld < B");
+  CK(cudaSetDevice(h->device));
+  if (imu_state && !is_device_ptr(imu_state)) return fail(A1MPC_EINVAL, "imu_state must be device memory (a1mpc_device_alloc)");
+  // x0 rows 0-2 (root_euler) and 6-8 (root_ang_vel) are two arrays: the rows in between belong to the estimator
+  double* euler = x0;
+  double* ang_vel = x0 ? x0 + 6 * ld : nullptr;
+  Stage st(h, B);
+  st.in(quat, 4); st.in(gyro, 3); st.in(acc, 3);
+  st.out(rot, 9, 8, ld); st.out(rot_z, 9, 8, ld); st.out(euler, 3, 8, ld); st.out(ang_vel, 3, 8, ld);
+  st.out(imu_acc, 3); st.out(imu_ang_vel, 3);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  const size_t kld = st.host() ? (size_t)B : ld;
+  CK(orientation_launch(B, quat, gyro, acc, static_cast<double*>(imu_state), rot, rot_z, euler, ang_vel, kld, imu_acc, imu_ang_vel, h->stream));
+  h->launches++;
+  return st.finish();
+}
+
+size_t a1mpc_command_bytes(int B) { return B > 0 ? (size_t)B * command_state_doubles() * sizeof(double) : 0; }
+
+int a1mpc_command_init_batch(a1mpc_handle* h, int B, void* cmd_state, const a1mpc_command_params* cp, double* ref, size_t ref_ld) {
+  if (!h || !cmd_state || !cp) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (ref && ref_ld < (size_t)B) return fail(A1MPC_EINVAL, "ref_ld must be >= B");
+  if (cp->variant != A1MPC_VARIANT_GAZEBO && cp->variant != A1MPC_VARIANT_HARDWARE && cp->variant != A1MPC_VARIANT_ISAAC)
+    return fail(A1MPC_EINVAL, "unknown variant");
+  if (!(cp->body_height_min <= cp->body_height_max)) return fail(A1MPC_EINVAL, "body_height_min must not exceed body_height_max");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(cmd_state)) return fail(A1MPC_EINVAL, "cmd_state must be device memory (a1mpc_device_alloc)");
+  Stage st(h, B);
+  st.out(ref, 9, 8, ref_ld);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  CK(command_init_launch(B, *cp, static_cast<double*>(cmd_state), ref, st.host() ? (size_t)B : ref_ld, h->stream));
+  h->launches++;
+  return st.finish();
+}
+
+int a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, const double* cmd, const double* root_pos, size_t root_pos_ld,
+                        uint32_t* movement_mode, double* kp_linear, double* ref, size_t ref_ld, double* des, size_t stance_ld) {
+  if (!h || !cmd_state || !cmd || !root_pos || !movement_mode || !kp_linear) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (!(dt > 0.0)) return fail(A1MPC_EINVAL, "dt must be positive");
+  if (root_pos_ld < (size_t)B || stance_ld < (size_t)B || (ref && ref_ld < (size_t)B)) return fail(A1MPC_EINVAL, "ld < B");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(cmd_state)) return fail(A1MPC_EINVAL, "cmd_state must be device memory (a1mpc_device_alloc)");
+  Stage st(h, B);
+  st.in(cmd, 7); st.in(root_pos, 3, 8, root_pos_ld);
+  st.out(movement_mode, 1); st.out(kp_linear, 3, 8, stance_ld); st.inout(ref, 9, 8, ref_ld); st.out(des, 12, 8, stance_ld);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  const bool hm = st.host();
+  CK(command_launch(B, dt, static_cast<double*>(cmd_state), cmd, root_pos, hm ? (size_t)B : root_pos_ld, movement_mode, kp_linear, ref,
+                    hm ? (size_t)B : ref_ld, des, hm ? (size_t)B : stance_ld, h->stream));
+  h->launches++;
   return st.finish();
 }
 

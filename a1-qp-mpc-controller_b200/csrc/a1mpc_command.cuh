@@ -1,0 +1,209 @@
+// a1mpc_command.cuh -- the first two stages of a control tick, batched, with the adapters' own state on the device:
+//   * the orientation stage of the robot adapters (GazeboA1ROS.cpp:235-299, HardwareA1ROS.cpp:262-276, IsaacA1ROS.cpp:183-241):
+//     root_rot_mat = root_quat.toRotationMatrix(), root_euler = Utils::quat_to_euler(root_quat) (utils/Utils.cpp:7-32),
+//     root_rot_mat_z = AngleAxisd(yaw, UnitZ), root_ang_vel = root_rot_mat * imu_ang_vel, with the 5-sample MovingWindowFilters
+//     of the Gazebo / Isaac IMU callbacks in front
+//   * the command stage, main_update's front half (GazeboA1ROS.cpp:117-188, HardwareA1ROS.cpp:98-158, IsaacA1ROS.cpp:75-137):
+//     body height, walking toggle, desired velocities and euler angles, movement_mode, xy position lock
+// Include from exactly one translation unit (a1mpc_command.cu) -- and from tests/emu (g++, A1MPC_EMU).
+//
+// Both states are batch-major like the swing state (field f of robot b at state[f * B + b]), so a buffer is bound to the B it was
+// initialised for.  One thread per robot: a few dozen flops over a few dozen doubles, every load and store coalesced.
+#pragma once
+#include "a1mpc_filter.cuh"
+
+namespace a1mpc {
+
+// IMU state (a1mpc_imu_bytes): six MovingWindowFilter(5) (GazeboA1ROS.cpp:100-105, IsaacA1ROS.cpp:62-67), k = acc x,y,z, gyro x,y,z.
+// IM_FHDR + 4k + {0,1,2,3}: sum, Neumaier correction, fill count, ring head of filter k;  IM_FVAL + 5k + j: window slot j.
+constexpr int IM_WINDOW = 5;
+constexpr int IM_FHDR = 0, IM_FVAL = 24;
+constexpr int IM_FIELDS = IM_FVAL + 6 * IM_WINDOW;   // 54 doubles per robot
+
+// command state (a1mpc_command_bytes): the adapter's joystick state and the A1CtrlStates fields main_update carries from tick to
+// tick, plus the init-time parameters of the robot.
+// prev_joy_cmd_ctrl_state is not kept: main_update sets it from joy_cmd_ctrl_state before the toggle and reads it only in the same
+// call, so it lives in a register.
+constexpr int CM_HEIGHT = 0, CM_CTRL = 1;                    // joy_cmd_body_height, joy_cmd_ctrl_state
+constexpr int CM_EUL = 2, CM_POS = 5, CM_KP = 8, CM_LVD = 11;   // root_euler_d[3], root_pos_d[3], kp_linear[3], root_lin_vel_d[3]
+constexpr int CM_HMIN = 14, CM_HMAX = 15, CM_LOCK = 16, CM_VARIANT = 18;   // height limits, kp_linear_lock_{x,y}, adapter variant
+constexpr int CM_FIELDS = 19;
+constexpr int CM_GAZEBO = 0, CM_HARDWARE = 1, CM_ISAAC = 2;   // A1MPC_VARIANT_* of include/a1mpc.h
+
+struct CommandInit {
+  double height, hmin, hmax;   // initial joy_cmd_body_height, JOY_CMD_BODY_HEIGHT_MIN / _MAX
+  double kp[3], lock[2];       // initial kp_linear, kp_linear_lock_{x,y}
+  int variant;
+};
+
+__global__ void imu_init_kernel(int B, double* __restrict__ state) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  for (int f = 0; f < IM_FIELDS; ++f) state[(size_t)f * B + b] = 0.0;
+}
+
+// one IMU sample and one pose per robot, thread per robot.  quat [4][B] (w, x, y, z), gyro / acc [3][B] and imu_acc / imu_ang_vel
+// [3][B] have leading dimension B; rot, rot_z [9][B], euler and ang_vel [3][B] (rows 0-2 and 6-8 of x0) leading dimension ld.  imu
+// (the filter state), acc and every output may be null.
+__global__ void orientation_kernel(int B, const double* __restrict__ quat, const double* __restrict__ gyro, const double* __restrict__ acc,
+                                   double* __restrict__ imu, double* __restrict__ rot, double* __restrict__ rot_z, double* __restrict__ euler,
+                                   double* __restrict__ ang_vel, size_t ld, double* __restrict__ imu_acc, double* __restrict__ imu_ang_vel) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const size_t lb = (size_t)B;
+  double* s = imu ? imu + b : nullptr;
+  // imu_callback (GazeboA1ROS.cpp:282-299, IsaacA1ROS.cpp:224-241): filter k of window 5, or the raw sample (HardwareA1ROS.cpp:273-274)
+  double g[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    double v = gyro[a * lb + b];
+    if (s) v = mw_filter(s, lb, IM_WINDOW, IM_FVAL + IM_WINDOW * (3 + a), IM_FHDR + 4 * (3 + a), v);
+    g[a] = v;
+    if (imu_ang_vel) imu_ang_vel[a * lb + b] = v;
+  }
+  if (acc) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      double v = acc[a * lb + b];
+      if (s) v = mw_filter(s, lb, IM_WINDOW, IM_FVAL + IM_WINDOW * a, IM_FHDR + 4 * a, v);
+      if (imu_acc) imu_acc[a * lb + b] = v;
+    }
+  }
+  const double w = quat[b], x = quat[lb + b], y = quat[2 * lb + b], z = quat[3 * lb + b];   // used as given: no normalisation
+  // Eigen's QuaternionBase::toRotationMatrix
+  const double tx = 2.0 * x, ty = 2.0 * y, tz = 2.0 * z;
+  const double twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
+  const double R[9] = {1.0 - (tyy + tzz), txy - twz, txz + twy, txy + twz, 1.0 - (txx + tzz), tyz - twx, txz - twy, tyz + twx, 1.0 - (txx + tyy)};
+  if (rot) {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) rot[k * ld + b] = R[k];
+  }
+  // Utils::quat_to_euler (utils/Utils.cpp:7-32): roll, pitch (t2 clamped to +-1), yaw
+  const double ysq = y * y;
+  const double t0 = 2.0 * (w * x + y * z), t1 = 1.0 - 2.0 * (x * x + ysq);
+  double t2 = 2.0 * (w * y - z * x);
+  t2 = t2 > 1.0 ? 1.0 : t2;
+  t2 = t2 < -1.0 ? -1.0 : t2;
+  const double t3 = 2.0 * (w * z + x * y), t4 = 1.0 - 2.0 * (ysq + z * z);
+  const double yaw = atan2(t3, t4);
+  if (euler) {
+    euler[b] = atan2(t0, t1);
+    euler[ld + b] = asin(t2);
+    euler[2 * ld + b] = yaw;
+  }
+  // Eigen's AngleAxis::toRotationMatrix about UnitZ: cos / sin of the full angle, diagonal (1 - c) * axis .* axis + c
+  if (rot_z) {
+    double sn, c;
+    sincos(yaw, &sn, &c);
+    const double Z[9] = {c, 0.0 - sn, 0.0, 0.0 + sn, c, 0.0, 0.0, 0.0, (1.0 - c) + c};
+#pragma unroll
+    for (int k = 0; k < 9; ++k) rot_z[k * ld + b] = Z[k];
+  }
+  // root_ang_vel = root_rot_mat * imu_ang_vel with the rotation of this call
+  if (ang_vel) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) ang_vel[i * ld + b] = R[3 * i] * g[0] + R[3 * i + 1] * g[1] + R[3 * i + 2] * g[2];
+  }
+}
+
+// the adapters' constructor values (GazeboA1ROS.cpp:60-62, GazeboA1ROS.h:130) and A1CtrlStates::reset() / resetFromROSParam()
+// (A1CtrlStates.h:35-36, 270-301); ref (may be null) gets the reset values of its nine rows.
+__global__ void command_init_kernel(int B, CommandInit P, double* __restrict__ state, double* __restrict__ ref, size_t ref_ld) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const size_t lb = (size_t)B;
+  double* s = state + b;
+  for (int f = 0; f < CM_FIELDS; ++f) s[f * lb] = 0.0;
+  s[CM_HEIGHT * lb] = P.height;
+  s[CM_HMIN * lb] = P.hmin;
+  s[CM_HMAX * lb] = P.hmax;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) s[(CM_KP + a) * lb] = P.kp[a];
+  s[CM_LOCK * lb] = P.lock[0];
+  s[(CM_LOCK + 1) * lb] = P.lock[1];
+  s[CM_VARIANT * lb] = (double)P.variant;
+  if (ref) {
+#pragma unroll
+    for (int r = 0; r < 9; ++r) ref[r * ref_ld + b] = 0.0;
+  }
+}
+
+// main_update's front half (GazeboA1ROS.cpp:122-188; HardwareA1ROS.cpp:104-158; IsaacA1ROS.cpp:81-137), thread per robot.
+// cmd [7][B]: velx, vely, velz, roll rate, pitch rate, yaw rate, toggle request.  root_pos [3][pos_ld]; kp [3][des_ld], des [12][des_ld]
+// (may be null), ref [9][ref_ld] (may be null: then root_euler_d[1] comes from the state).
+__global__ void command_kernel(int B, double dt, double* __restrict__ state, const double* __restrict__ cmd, const double* __restrict__ root_pos,
+                               size_t pos_ld, uint32_t* __restrict__ movement_mode, double* __restrict__ kp, double* __restrict__ ref, size_t ref_ld,
+                               double* __restrict__ des, size_t des_ld) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const size_t lb = (size_t)B;
+  double* s = state + b;
+  double c[7];
+#pragma unroll
+  for (int k = 0; k < 7; ++k) c[k] = cmd[k * lb + b];
+  const int variant = (int)s[CM_VARIANT * lb];
+  const bool hw = variant == CM_HARDWARE;
+  // body height integrated and clamped (:122-130)
+  double h = s[CM_HEIGHT * lb] + c[2] * dt;
+  if (h >= s[CM_HMAX * lb]) h = s[CM_HMAX * lb];
+  if (h <= s[CM_HMIN * lb]) h = s[CM_HMIN * lb];
+  // walking toggle (:140-147)
+  const int prev = (int)s[CM_CTRL * lb];
+  int ctrl = prev;
+  if (c[6] != 0.0) ctrl = (ctrl + 1) % 2;
+  // desired velocities (:149-157).  Only Gazebo sets root_lin_vel_d[2] = velz (GazeboA1ROS.cpp:152); the hardware and Isaac
+  // adapters set x and y only (HardwareA1ROS.cpp:121-123, IsaacA1ROS.cpp:99-101) and leave z at its reset value
+  double lvd[3] = {c[0], c[1], variant == CM_GAZEBO ? c[2] : s[(CM_LVD + 2) * lb]};
+  // desired euler angles (:158-160).  root_euler_d[1] starts from row 1 of ref when given: compute_grf's terrain adaptation
+  // overwrites it there (A1RobotControl.cpp:358-364) and the next tick integrates on top of that value.  The hardware adapter
+  // assigns the roll and pitch rates themselves (HardwareA1ROS.cpp:129-130).
+  double e[3], p[3], k[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) { e[a] = s[(CM_EUL + a) * lb]; p[a] = s[(CM_POS + a) * lb]; k[a] = s[(CM_KP + a) * lb]; }
+  if (ref) e[1] = ref[ref_ld + b];
+  if (hw) {
+    e[0] = c[3];
+    e[1] = c[4];
+  } else {
+    e[0] += c[3] * dt;
+    e[1] += c[4] * dt;
+  }
+  e[2] += c[5] * dt;
+  p[2] = h;
+  // movement mode and the xy position lock (:163-188)
+  uint32_t mode = 0;
+  if (ctrl == 1) {
+    mode = 1;
+  } else if (ctrl == 0 && prev == 1) {
+    p[0] = root_pos[b]; p[1] = root_pos[pos_ld + b];
+    k[0] = s[CM_LOCK * lb]; k[1] = s[(CM_LOCK + 1) * lb];
+  }
+  if (mode == 1) {
+    if (sqrt(lvd[0] * lvd[0] + lvd[1] * lvd[1]) > 0.05) {
+      p[0] = root_pos[b]; p[1] = root_pos[pos_ld + b];
+      k[0] = 0.0; k[1] = 0.0;
+    } else {
+      k[0] = s[CM_LOCK * lb]; k[1] = s[(CM_LOCK + 1) * lb];
+    }
+  }
+  s[CM_HEIGHT * lb] = h;
+  s[CM_CTRL * lb] = (double)ctrl;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    s[(CM_EUL + a) * lb] = e[a]; s[(CM_POS + a) * lb] = p[a]; s[(CM_KP + a) * lb] = k[a]; s[(CM_LVD + a) * lb] = lvd[a];
+    kp[a * des_ld + b] = k[a];
+  }
+  movement_mode[b] = mode;
+  if (ref) {   // root_euler_d[0..1], root_ang_vel_d, root_lin_vel_d (body), root_pos_d[2]
+    const double r[9] = {e[0], e[1], c[3], c[4], c[5], lvd[0], lvd[1], lvd[2], p[2]};
+#pragma unroll
+    for (int i = 0; i < 9; ++i) ref[i * ref_ld + b] = r[i];
+  }
+  if (des) {   // root_euler_d, root_pos_d, root_lin_vel_d (body), root_ang_vel_d
+    const double d[12] = {e[0], e[1], e[2], p[0], p[1], p[2], lvd[0], lvd[1], lvd[2], c[3], c[4], c[5]};
+#pragma unroll
+    for (int i = 0; i < 12; ++i) des[i * des_ld + b] = d[i];
+  }
+}
+
+}  // namespace a1mpc

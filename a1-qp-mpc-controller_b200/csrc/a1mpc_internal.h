@@ -52,4 +52,14 @@ cudaError_t stance_qp_launch(int sm_count, int B, size_t ld, const double* x0, c
                              const uint32_t* contact, const double* des, const double* kp_linear, const double* gains9, double mass,
                              double* f_body, int32_t* status, double* root_acc, void* scratch, cudaStream_t st, int* nlaunch);
 
+// orientation and command stages (a1mpc_command.cu, kernels in a1mpc_command.cuh), thread per robot on the stream
+size_t imu_state_doubles();       // per robot
+size_t command_state_doubles();   // per robot
+cudaError_t imu_init_launch(int B, double* state, cudaStream_t st);
+cudaError_t orientation_launch(int B, const double* quat, const double* gyro, const double* acc, double* imu, double* rot, double* rot_z,
+                               double* euler, double* ang_vel, size_t ld, double* imu_acc, double* imu_ang_vel, cudaStream_t st);
+cudaError_t command_init_launch(int B, const a1mpc_command_params& cp, double* state, double* ref, size_t ref_ld, cudaStream_t st);
+cudaError_t command_launch(int B, double dt, double* state, const double* cmd, const double* root_pos, size_t pos_ld, uint32_t* movement_mode,
+                           double* kp, double* ref, size_t ref_ld, double* des, size_t des_ld, cudaStream_t st);
+
 }  // namespace a1mpc

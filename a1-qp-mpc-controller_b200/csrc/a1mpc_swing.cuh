@@ -16,6 +16,7 @@
 // early-contact mask, and the terrain stage needs all four legs at once; batch-major fields keep every load and store coalesced.
 #pragma once
 #include "a1mpc_device.cuh"
+#include "a1mpc_filter.cuh"
 
 namespace a1mpc {
 
@@ -33,32 +34,9 @@ struct SwingParams {
   double kp[12], kd[12];   // kp_foot, kd_foot leg-major: [3 leg + axis]
 };
 
-// MovingWindowFilter::CalculateAverage (utils/filter.hpp:26-39) on filter k of the robot whose state starts at s (stride ld):
-// once the window is full the oldest value is subtracted BEFORE the new one is added, both by Neumaier's compensated sum, and the
-// average always divides by the full window size (biased towards 0 while filling).
-__device__ __forceinline__ void sw_neumaier(double& sum, double& corr, double v) {
-  const double ns = sum + v;
-  if (fabs(sum) >= fabs(v)) corr += (sum - ns) + v;
-  else corr += (v - ns) + sum;
-  sum = ns;
-}
+// filter k of the robot whose swing state starts at s (stride ld)
 __device__ __forceinline__ double sw_filter(double* s, size_t ld, int k, double x) {
-  const int W = k < 12 ? SW_RC_WINDOW : SW_TA_WINDOW;
-  double* val = s + (size_t)(SW_FVAL + SW_RC_WINDOW * k) * ld;
-  double* hd = s + (size_t)(SW_FHDR + 4 * k) * ld;
-  double sum = hd[0], corr = hd[ld];
-  int cnt = (int)hd[2 * ld], head = (int)hd[3 * ld];
-  if (cnt < W) {
-    val[(size_t)cnt * ld] = x;
-    ++cnt;
-  } else {
-    sw_neumaier(sum, corr, -val[(size_t)head * ld]);
-    val[(size_t)head * ld] = x;
-    head = head + 1 == W ? 0 : head + 1;
-  }
-  sw_neumaier(sum, corr, x);
-  hd[0] = sum; hd[ld] = corr; hd[2 * ld] = (double)cnt; hd[3 * ld] = (double)head;
-  return (sum + corr) / (double)W;
+  return mw_filter(s, ld, k < 12 ? SW_RC_WINDOW : SW_TA_WINDOW, SW_FVAL + SW_RC_WINDOW * k, SW_FHDR + 4 * k, x);
 }
 
 // BezierUtils::bezier_curve (utils/Utils.cpp:100-107), degree 4: sum_i C(4,i) t^i (1-t)^(4-i) P_i accumulated in index order.  The

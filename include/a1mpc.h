@@ -28,8 +28,8 @@
  *           the call is synchronous.
  *   device  the call only enqueues on the handle's stream (a1mpc_sync) and copies nothing.
  * The batch-uniform parameters that a call reads itself (km_foot, torques_gravity, rho_opt, rho_fix,
- * kp_foot, kd_foot, kd_linear, kp_angular, kd_angular) are always host memory, and the state buffers (warm, ekf_state, swing_state)
- * always device memory; A1MPC_EINVAL otherwise.
+ * kp_foot, kd_foot, kd_linear, kp_angular, kd_angular, the command params) are always host memory, and the state buffers (warm,
+ * ekf_state, swing_state, imu_state, cmd_state) always device memory; A1MPC_EINVAL otherwise.
  */
 #ifndef A1MPC_H_
 #define A1MPC_H_
@@ -337,6 +337,76 @@ int  a1mpc_swing_legs_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp,
                             double* foot_pos_recent_contact);
 int  a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref, size_t ref_ld,
                                double* terrain_pitch);
+
+/* ---- the first two stages of a control tick: the adapters' orientation and command stages ---------------------------------
+ * Together with the stages above they let a whole tick run from raw sensor arrays on device pointers.  One thread per robot;
+ * batch-major SoA, host or device arrays; the state buffers are device memory (a1mpc_device_alloc), opaque and batch-major, so a
+ * buffer is bound to the B it was initialised for.
+ *
+ * a1mpc_orientation_batch: the IMU and pose callbacks (GazeboA1ROS.cpp:235-299, HardwareA1ROS.cpp:262-276, IsaacA1ROS.cpp:183-241).
+ *   quat [4][B] (w, x, y, z: the Quaterniond(w, x, y, z) argument order), gyro [3][B], acc [3][B] (may be NULL): the raw readings.
+ *   imu_state  a1mpc_imu_bytes(B) bytes, a1mpc_imu_init_batch: the six MovingWindowFilter(5) of acc and gyro (GazeboA1ROS.cpp:100-105,
+ *              IsaacA1ROS.cpp:62-67; utils/filter.hpp), through which each call first passes its sample.  NULL = unfiltered, as on
+ *              the hardware adapter (HardwareA1ROS.cpp:273-274).
+ *   outputs, each may be NULL:
+ *     rot [9][ld], rot_z [9][ld]   root_rot_mat = quat.toRotationMatrix() and root_rot_mat_z = AngleAxisd(yaw, UnitZ), row-major
+ *     x0 [12][ld]                  only rows 0-2 (root_euler = Utils::quat_to_euler, utils/Utils.cpp:7-32) and rows 6-8
+ *                                  (root_ang_vel = root_rot_mat * imu_ang_vel, world) are written; rows 3-5 and 9-11 belong to the
+ *                                  estimator.  With ld the x0 and rot of an a1mpc_inputs pass as they are.
+ *                                  ld applies to rot, rot_z and x0 alike: a1mpc_stance_qp_batch takes rot_z with its ld, but
+ *                                  a1mpc_update_plan_batch and a1mpc_swing_legs_batch take a dense rot_z [9][B], so with ld > B
+ *                                  write rot_z with a second call (ld = B) or into a separate dense array for them.
+ *     imu_acc [3][B], imu_ang_vel [3][B]   the (filtered) readings, as a1mpc_ekf_update_batch takes them; imu_acc needs acc.
+ *   As the reference computes it, not as it means it: the quaternion is NOT normalised (Eigen's toRotationMatrix and quat_to_euler
+ *   use the raw coefficients); the pitch argument t2 is clamped to +-1 before asin; rot_z is Eigen's AngleAxis matrix of the yaw that
+ *   quat_to_euler returned (cos / sin of the full angle, diagonal element (1 - c) + c).  One difference in timing: Gazebo computes
+ *   root_ang_vel in the IMU callback with whatever rotation the last pose message left, Isaac in the pose callback with the last gyro
+ *   sample; here it always uses the rotation and the gyro sample of the same call.
+ *
+ * a1mpc_command_batch: main_update's front half (GazeboA1ROS.cpp:117-188, HardwareA1ROS.cpp:98-158, IsaacA1ROS.cpp:75-137).
+ *   cmd_state  a1mpc_command_bytes(B) bytes: joy_cmd_body_height, joy_cmd_ctrl_state, root_euler_d,
+ *              root_pos_d, kp_linear, root_lin_vel_d and the init parameters.  a1mpc_command_init_batch sets it from cp (batch-uniform):
+ *              body_height = the adapter's initial joy_cmd_body_height (0.3 Gazebo, 0.12 hardware, 0.32 Isaac: GazeboA1ROS.h:130,
+ *              HardwareA1ROS.h:107, IsaacA1ROS.h:80), the clamp JOY_CMD_BODY_HEIGHT_MIN / _MAX (0.1 / 0.32, A1Params.h:16-17),
+ *              kp_linear and kp_linear_lock (120, 120, 500 / 120, 120 from the ROS-parameter defaults, A1CtrlStates.h:270-301) and
+ *              the adapter variant; control state 0, everything else zero (A1CtrlStates::reset).  Its ref (may be NULL, ref_ld >= B)
+ *              gets those reset values in all nine rows, which is what the first command call reads back (below).
+ *   cmd [7][B]  per robot, in physical units (what joy_callback leaves after its axis scaling): velx, vely, velz, roll rate, pitch
+ *               rate, yaw rate, toggle request (non-zero = toggle walking).
+ *   root_pos [3][root_pos_ld]  the previous estimate (A1BasicEKF.cpp:162): x0 + 3 ld of an a1mpc_inputs passes as it is.
+ *   Per tick: height += velz dt, clamped; the walking toggle; root_lin_vel_d.xy = (velx, vely); root_ang_vel_d = the three rates;
+ *   root_euler_d[0..1] += rate dt; root_euler_d[2] += yaw rate dt; root_pos_d[2] = height; movement_mode = walking; the step out of
+ *   walking locks root_pos_d.xy = root_pos.xy with the lock gains; while walking |root_lin_vel_d.xy| > 0.05 refreshes
+ *   root_pos_d.xy = root_pos.xy and zeroes kp_linear.xy, otherwise kp_linear.xy = the lock gains.  The variants differ where the
+ *   adapters differ, reproduced literally: only Gazebo sets root_lin_vel_d[2] = velz (GazeboA1ROS.cpp:152); the hardware and Isaac
+ *   adapters set x and y only and leave it at 0 (HardwareA1ROS.cpp:121-123, IsaacA1ROS.cpp:99-101).  A1MPC_VARIANT_HARDWARE
+ *   also ASSIGNS root_euler_d[0..1] the roll and pitch rates instead of integrating them (HardwareA1ROS.cpp:129-130).
+ *   outputs: movement_mode [B] (the layout of a1mpc_update_plan_batch / a1mpc_ekf_update_batch); kp_linear [3][stance_ld] and des
+ *   [12][stance_ld] (may be NULL) in the layout of a1mpc_stance_qp_batch (its ld); ref [9][ref_ld] (may be NULL) in the a1mpc_inputs
+ *   layout, so root_lin_vel_d is ref + 5 ref_ld for a1mpc_update_plan_batch.
+ *   The pitch round trip: compute_grf's terrain adaptation overwrites root_euler_d[1] (a1mpc_terrain_pitch_batch writes row 1 of ref,
+ *   A1RobotControl.cpp:358-364) and the next main_update integrates on top of it.  So when ref is given, this tick's root_euler_d[1]
+ *   starts from what row 1 of ref holds; without ref it starts from the state.  Pass the same ref to a1mpc_command_init_batch (or
+ *   hold 0 in its row 1) before the first call.
+ * A1MPC_EINVAL: NULL handle, state or mandatory array, B <= 0, an ld < B, a state buffer that is not device memory, unknown variant. */
+#define A1MPC_VARIANT_GAZEBO   0
+#define A1MPC_VARIANT_HARDWARE 1
+#define A1MPC_VARIANT_ISAAC    2
+typedef struct a1mpc_command_params {
+  int    variant;               /* A1MPC_VARIANT_* */
+  double body_height;           /* initial joy_cmd_body_height */
+  double body_height_min, body_height_max;
+  double kp_linear[3];          /* initial kp_linear */
+  double kp_linear_lock[2];     /* kp_linear_lock_x, _y */
+} a1mpc_command_params;
+size_t a1mpc_imu_bytes(int B);
+int  a1mpc_imu_init_batch(a1mpc_handle* h, int B, void* imu_state);
+int  a1mpc_orientation_batch(a1mpc_handle* h, int B, const double* quat, const double* gyro, const double* acc, void* imu_state, double* rot,
+                             double* rot_z, double* x0, size_t ld, double* imu_acc, double* imu_ang_vel);
+size_t a1mpc_command_bytes(int B);
+int  a1mpc_command_init_batch(a1mpc_handle* h, int B, void* cmd_state, const a1mpc_command_params* cp, double* ref, size_t ref_ld);
+int  a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, const double* cmd, const double* root_pos, size_t root_pos_ld,
+                         uint32_t* movement_mode, double* kp_linear, double* ref, size_t ref_ld, double* des, size_t stance_ld);
 
 /* ---- device memory, stream and timing helpers (so hosts need no CUDA headers) -------------- */
 int  a1mpc_device_alloc(a1mpc_handle* h, size_t bytes, void** ptr);
