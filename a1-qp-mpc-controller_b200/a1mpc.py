@@ -7,6 +7,7 @@ A1RobotControlBatch shims under host/) directly.
 """
 import ctypes as C
 import os
+import weakref
 
 import numpy as np
 
@@ -21,6 +22,7 @@ EXPORTS = [
     "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
     "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch",
     "a1mpc_imu_bytes", "a1mpc_imu_init_batch", "a1mpc_orientation_batch", "a1mpc_command_bytes", "a1mpc_command_init_batch", "a1mpc_command_batch",
+    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_run", "a1mpc_tick_destroy",
     "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
@@ -75,6 +77,35 @@ def default_command_params(variant=VARIANT_GAZEBO):
     c.kp_linear[:] = [120.0, 120.0, 500.0]
     c.kp_linear_lock[:] = [120.0, 120.0]
     return c
+
+
+TICK_QP, TICK_MPC = 0, 1
+
+
+class TickParams(C.Structure):
+    _fields_ = [("mode", C.c_int), ("use_terrain_adapt", C.c_int), ("assume_flat_ground", C.c_int), ("gait", GaitParams), ("command", CommandParams),
+                ("rho_opt", C.c_double * 12), ("rho_fix", C.c_double * 20), ("kp_foot", C.c_double * 12), ("kd_foot", C.c_double * 12),
+                ("km_foot", C.c_double * 3), ("torques_gravity", C.c_double * 12), ("kd_linear", C.c_double * 3), ("kp_angular", C.c_double * 3),
+                ("kd_angular", C.c_double * 3)]
+
+
+TICK_INPUTS = ("quat", "gyro", "acc", "joint_pos", "joint_vel", "foot_force", "cmd", "gait_counter_speed")
+TICK_OUTPUTS = ("tau", "f_body", "status", "contacts", "movement_mode", "x0", "ref")
+
+
+class TickInputs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in TICK_INPUTS]
+
+
+class TickOutputs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in TICK_OUTPUTS]
+
+
+def default_tick_params(variant=VARIANT_GAZEBO, mode=TICK_MPC):
+    """a1mpc_default_tick_params: the reference's launch parameters of one adapter and stance_leg_control_type"""
+    tp = TickParams()
+    _check(lib().a1mpc_default_tick_params(variant, mode, C.byref(tp)))
+    return tp
 
 
 class InputsExt(C.Structure):
@@ -153,6 +184,11 @@ def lib():
         l.a1mpc_command_init_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(CommandParams), C.c_void_p, C.c_size_t]
         l.a1mpc_command_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+        l.a1mpc_default_tick_params.argtypes = [C.c_int, C.c_int, C.POINTER(TickParams)]
+        l.a1mpc_tick_create.argtypes = [C.c_void_p, C.c_int, C.POINTER(TickParams), C.POINTER(C.c_void_p)]
+        l.a1mpc_tick_reset.argtypes = [C.c_void_p]
+        l.a1mpc_tick_run.argtypes = [C.c_void_p, C.c_double, C.POINTER(TickInputs), C.POINTER(TickOutputs)]
+        l.a1mpc_tick_destroy.argtypes = [C.c_void_p]
         l.a1mpc_gen_states.argtypes = [C.c_int, C.c_uint64, C.c_int] + [C.c_void_p] * 5
         l.a1mpc_measure_fp64_peak.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         l.a1mpc_profile_begin.argtypes = [C.c_void_p, C.c_int]
@@ -242,6 +278,59 @@ class DeviceBatch:
                 setattr(self, name, None)
 
 
+class Tick:
+    """a whole control tick for B robots (a1mpc_tick_*): owns the controller state; raw sensor arrays in, joint torques out"""
+
+    _SHAPES = dict(quat=(4,), gyro=(3,), acc=(3,), joint_pos=(12,), joint_vel=(12,), foot_force=(4,), cmd=(7,), gait_counter_speed=(4,))
+
+    def __init__(self, eng, B, params=None):
+        self.eng, self.B = eng, B
+        self.params = params if params is not None else default_tick_params()
+        t = C.c_void_p()
+        _check(lib().a1mpc_tick_create(eng.h, B, C.byref(self.params), C.byref(t)))
+        self.t = t
+        eng._ticks.add(self)   # Engine.close destroys its ticks first: a tick must go before its handle
+
+    def run(self, dt, quat, gyro, acc, joint_pos, joint_vel, foot_force, cmd, gait_counter_speed):
+        """one tick on host arrays ([rows][B] float64) -> (tau [12][B], dict of f_body, status, contacts, movement_mode, x0 and, in MPC
+        mode, ref)"""
+        B = self.B
+        args = dict(quat=quat, gyro=gyro, acc=acc, joint_pos=joint_pos, joint_vel=joint_vel, foot_force=foot_force, cmd=cmd,
+                    gait_counter_speed=gait_counter_speed)
+        arrs = {}
+        for k, a in args.items():
+            arrs[k] = np.ascontiguousarray(a, dtype=np.float64)
+            if arrs[k].shape != self._SHAPES[k] + (B,):
+                raise ValueError("%s must have shape %s" % (k, self._SHAPES[k] + (B,)))
+        outs = dict(tau=np.zeros((12, B)), f_body=np.zeros((12, B)), status=np.zeros(B, dtype=np.int32), contacts=np.zeros(B, dtype=np.uint32),
+                    movement_mode=np.zeros(B, dtype=np.uint32), x0=np.zeros((12, B)))
+        if self.params.mode == TICK_MPC:
+            outs["ref"] = np.zeros((9, B))
+        self.run_ptrs(dt, TickInputs(*[arrs[k].ctypes.data for k in TICK_INPUTS]),
+                      TickOutputs(*[outs[k].ctypes.data if k in outs else None for k in TICK_OUTPUTS]))
+        tau = outs.pop("tau")
+        return tau, outs
+
+    def run_ptrs(self, dt, inputs, outputs):
+        """one tick on a TickInputs / TickOutputs of device pointers (asynchronous on the handle's stream) or host pointers"""
+        _check(lib().a1mpc_tick_run(self.t, dt, C.byref(inputs), C.byref(outputs)))
+
+    def reset(self):
+        _check(lib().a1mpc_tick_reset(self.t))
+
+    def close(self):
+        """a1mpc_tick_destroy; a tick whose Engine is closed has already been destroyed by Engine.close"""
+        if self.t and self.eng.h:
+            lib().a1mpc_tick_destroy(self.t)
+        self.t = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Engine:
     """one handle = one H100 + one stream (a1mpc_create / a1mpc_destroy)"""
 
@@ -251,6 +340,7 @@ class Engine:
         _check(lib().a1mpc_create(C.byref(h), C.byref(self.cfg), device))
         self.h = h
         self.device = device
+        self._ticks = weakref.WeakSet()
 
     @property
     def ftype(self):
@@ -259,6 +349,8 @@ class Engine:
 
     def close(self):
         if self.h:
+            for tick in list(getattr(self, "_ticks", ())):
+                tick.close()
             lib().a1mpc_destroy(self.h)
             self.h = None
 

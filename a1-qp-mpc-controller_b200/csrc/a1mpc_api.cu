@@ -13,6 +13,7 @@
 #include "a1mpc_misc.cuh"
 #include "a1mpc_estim.cuh"
 #include "a1mpc_swing.cuh"
+#include "a1mpc_tick.cuh"
 
 using namespace a1mpc;
 
@@ -367,6 +368,24 @@ int solve_impl(a1mpc_handle* h, int B, const a1mpc_inputs* in, const a1mpc_input
   rc = ext ? enqueue_solve_ext(h, B, di, dsched, dnorm, dout, w, shift) : enqueue_solve(h, B, di, dout, w, shift);
   if (rc) return rc;
   return st.finish();
+}
+
+int enqueue_ekf_update(a1mpc_handle* h, int B, double* state, EkfParams P, const uint32_t* movement_mode, const double* imu_acc,
+                       const double* imu_ang_vel, const double* rot, const double* foot_pos_rel, const double* foot_vel_rel, const double* foot_force,
+                       double* root_pos, double* root_lin_vel, uint32_t* estimated_contacts, int32_t* status) {
+  static bool attr_set[64] = {};
+  const size_t smem = (size_t)EKF_WPC * EKF_WARP_DOUBLES * sizeof(double);
+  if (h->device < 64 && !attr_set[h->device]) {
+    CK(cudaFuncSetAttribute(ekf_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set[h->device] = true;
+  }
+  int grid = (B + EKF_WPC - 1) / EKF_WPC;
+  if (grid > h->sm_count * 2) grid = h->sm_count * 2;
+  ekf_update_kernel<<<grid, 32 * EKF_WPC, smem, h->stream>>>(B, P, state, movement_mode, imu_acc, imu_ang_vel, rot, foot_pos_rel, foot_vel_rel,
+                                                             foot_force, root_pos, root_lin_vel, estimated_contacts, status);
+  h->launches++;
+  CK(cudaGetLastError());
+  return A1MPC_OK;
 }
 
 }  // namespace
@@ -752,25 +771,15 @@ int a1mpc_ekf_update_batch(a1mpc_handle* h, int B, void* ekf_state, double dt, i
   if (!(dt > 0.0)) return fail(A1MPC_EINVAL, "dt must be positive");
   CK(cudaSetDevice(h->device));
   if (!is_device_ptr(ekf_state)) return fail(A1MPC_EINVAL, "ekf_state must be device memory (a1mpc_device_alloc)");
-  static bool attr_set[64] = {};
-  const size_t smem = (size_t)EKF_WPC * EKF_WARP_DOUBLES * sizeof(double);
-  if (h->device < 64 && !attr_set[h->device]) {
-    CK(cudaFuncSetAttribute(ekf_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set[h->device] = true;
-  }
   Stage st(h, B);
   st.in(movement_mode, 1); st.in(imu_acc, 3); st.in(imu_ang_vel, 3); st.in(rot, 9); st.in(foot_pos_rel, 12); st.in(foot_vel_rel, 12);
   st.in(foot_force, 4);
   st.out(root_pos, 3); st.out(root_lin_vel, 3); st.out(estimated_contacts, 1); st.out(status, 1);
   int rc;
   if ((rc = st.begin())) return rc;
-  EkfParams P{dt, assume_flat_ground ? 1 : 0};
-  int grid = (B + EKF_WPC - 1) / EKF_WPC;
-  if (grid > h->sm_count * 2) grid = h->sm_count * 2;
-  ekf_update_kernel<<<grid, 32 * EKF_WPC, smem, h->stream>>>(B, P, static_cast<double*>(ekf_state), movement_mode, imu_acc, imu_ang_vel, rot,
-                                                             foot_pos_rel, foot_vel_rel, foot_force, root_pos, root_lin_vel, estimated_contacts, status);
-  h->launches++;
-  CK(cudaGetLastError());
+  if ((rc = enqueue_ekf_update(h, B, static_cast<double*>(ekf_state), EkfParams{dt, assume_flat_ground ? 1 : 0}, movement_mode, imu_acc, imu_ang_vel, rot,
+                               foot_pos_rel, foot_vel_rel, foot_force, root_pos, root_lin_vel, estimated_contacts, status)))
+    return rc;
   return st.finish();
 }
 
@@ -914,6 +923,291 @@ int a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, cons
                     hm ? (size_t)B : ref_ld, des, hm ? (size_t)B : stance_ld, h->stream));
   h->launches++;
   return st.finish();
+}
+
+// ---- a whole control tick (a1mpc_tick_*) ---------------------------------------------------------------------------------------
+}  // extern "C"
+
+struct a1mpc_tick {
+  a1mpc_handle* h = nullptr;
+  int B = 0;
+  a1mpc_tick_params tp;
+  bool first = true;      // the next run initialises the EKF instead of updating it
+  void* mem = nullptr;    // one device allocation holding everything below
+  // intermediates, dense [rows][B]
+  double *rot, *rz, *x0, *ia, *ig, *fpr, *fvr, *jac, *foot, *kpl, *des, *ref, *fk, *f_body;
+  uint32_t *mode, *contact, *est_contacts;
+  int32_t *status, *est_status;
+  // state
+  double *gc, *tau, *imu, *cmd, *swing, *ekf;
+  uint32_t* warm;
+};
+
+namespace {
+
+int tick_reset_impl(a1mpc_tick* t) {
+  a1mpc_handle* h = t->h;
+  const int B = t->B;
+  const size_t lb = (size_t)B;
+  CK(cudaSetDevice(h->device));
+  CK(cudaMemsetAsync(t->x0, 0, 12 * lb * sizeof(double), h->stream));
+  CK(cudaMemsetAsync(t->gc, 0, 4 * lb * sizeof(double), h->stream));
+  CK(cudaMemsetAsync(t->tau, 0, 12 * lb * sizeof(double), h->stream));
+  if (t->imu) {
+    CK(imu_init_launch(B, t->imu, h->stream));
+    h->launches++;
+  }
+  const bool mpc = t->tp.mode == A1MPC_TICK_MPC;
+  CK(command_init_launch(B, t->tp.command, t->cmd, mpc ? t->ref : nullptr, lb, h->stream));
+  swing_init_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->swing);
+  h->launches += 2;
+  CK(cudaGetLastError());
+  if (t->warm) CK(cudaMemsetAsync(t->warm, 0, a1mpc_warm_bytes(h, B), h->stream));
+  t->first = true;
+  return A1MPC_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int a1mpc_default_tick_params(int variant, int mode, a1mpc_tick_params* tp) {
+  if (!tp) return fail(A1MPC_EINVAL, "null argument");
+  if (variant != A1MPC_VARIANT_GAZEBO && variant != A1MPC_VARIANT_HARDWARE && variant != A1MPC_VARIANT_ISAAC) return fail(A1MPC_EINVAL, "unknown variant");
+  if (mode != A1MPC_TICK_QP && mode != A1MPC_TICK_MPC) return fail(A1MPC_EINVAL, "unknown mode");
+  std::memset(tp, 0, sizeof(*tp));
+  const bool mpc = mode == A1MPC_TICK_MPC;
+  const int v = variant;   // 0 Gazebo, 1 hardware, 2 Isaac
+  tp->mode = mode;
+  // use_terrain_adapt: A1CtrlStates.h:137 (ROS default 1); isaac_a1_mpc.yaml:3 sets 0
+  tp->use_terrain_adapt = (v == A1MPC_VARIANT_ISAAC && mpc) ? 0 : 1;
+  // every adapter constructs A1BasicEKF a1_estimate (GazeboA1ROS.h:157, HardwareA1ROS.h:134, IsaacA1ROS.h:107): assume_flat_ground = true
+  // (A1BasicEKF.cpp:40)
+  tp->assume_flat_ground = 1;
+  // gait: counter_per_gait / _swing (A1CtrlStates.h:24-25), control_dt = MAIN_UPDATE_FREQUENCY / 1000 (A1CtrlStates.h:332, A1Params.h:11),
+  // FOOT_DELTA_{X,Y}_LIMIT (A1Params.h:44-45); default_foot_pos 3 x 4 row-major (x, y, z rows; FL, FR, RL, RR) from
+  // config/<variant>_a1_<mode>.yaml a1_default_foot_pos_* (gazebo_a1_mpc.yaml:17-31, gazebo_a1_qp.yaml:10-24, hardware_a1_mpc.yaml:18-32,
+  // hardware_a1_qp.yaml:11-25, isaac_a1_mpc.yaml:18-32, isaac_a1_qp.yaml:10-24)
+  tp->gait.counter_per_gait = 240.0;
+  tp->gait.counter_per_swing = 120.0;
+  tp->gait.control_dt = 2.5 / 1000.0;
+  tp->gait.foot_delta_x_limit = 0.1;
+  tp->gait.foot_delta_y_limit = 0.1;
+  tp->gait.horizon = 0;
+  {
+    const double front_x = v == A1MPC_VARIANT_ISAAC ? (mpc ? 0.24 : 0.25) : 0.17;
+    const double z = v == A1MPC_VARIANT_HARDWARE ? (mpc ? -0.3 : -0.33) : (v == A1MPC_VARIANT_ISAAC ? (mpc ? -0.35 : -0.33) : -0.35);
+    const double fp[12] = {front_x, front_x, -0.17, -0.17, 0.15, -0.15, 0.15, -0.15, z, z, z, z};
+    for (int i = 0; i < 12; ++i) tp->gait.default_foot_pos[i] = fp[i];
+  }
+  // command: the adapter's initial joy_cmd_body_height (GazeboA1ROS.h:130, HardwareA1ROS.h:107, IsaacA1ROS.h:80), JOY_CMD_BODY_HEIGHT_MIN /
+  // _MAX (A1Params.h:16-17); kp_linear = a1_kp_linear_* (A1CtrlStates.h:273-275, ROS defaults 120, 120, 500; the QP configs set them:
+  // gazebo_a1_qp.yaml:54-56, hardware_a1_qp.yaml:55-57, isaac_a1_qp.yaml:54-56) and kp_linear_lock = its x and y (A1CtrlStates.h:298-299)
+  tp->command.variant = variant;
+  tp->command.body_height = v == A1MPC_VARIANT_GAZEBO ? 0.3 : (v == A1MPC_VARIANT_HARDWARE ? 0.12 : 0.32);
+  tp->command.body_height_min = 0.1;
+  tp->command.body_height_max = 0.32;
+  {
+    static const double kpl_qp[3][3] = {{100.0, 100.0, 300.0}, {400.0, 400.0, 1500.0}, {1450.0, 1450.0, 3800.0}};
+    const double kpl_ros[3] = {120.0, 120.0, 500.0};
+    const double* kpl = mpc ? kpl_ros : kpl_qp[v];
+    for (int i = 0; i < 3; ++i) tp->command.kp_linear[i] = kpl[i];
+    tp->command.kp_linear_lock[0] = kpl[0];
+    tp->command.kp_linear_lock[1] = kpl[1];
+  }
+  // leg geometry (GazeboA1ROS.cpp:75-97, HardwareA1ROS.cpp:52-74, IsaacA1ROS.cpp:38-60): rho_opt = 0; rho_fix = leg_offset_x, leg_offset_y,
+  // motor_offset, upper_leg_length (0.21 Gazebo, 0.20 hardware, 0.22 Isaac), lower_leg_length (LOWER_LEG_LENGTH = 0.21, A1Params.h:36;
+  // 0.20 hardware)
+  {
+    const double upper = v == A1MPC_VARIANT_GAZEBO ? 0.21 : (v == A1MPC_VARIANT_HARDWARE ? 0.20 : 0.22);
+    const double lower = v == A1MPC_VARIANT_HARDWARE ? 0.20 : 0.21;
+    const double ox[4] = {0.1805, 0.1805, -0.1805, -0.1805}, oy[4] = {0.047, -0.047, 0.047, -0.047}, mo[4] = {0.0838, -0.0838, 0.0838, -0.0838};
+    for (int i = 0; i < 4; ++i) {
+      const double r[5] = {ox[i], oy[i], mo[i], upper, lower};
+      for (int k = 0; k < 5; ++k) tp->rho_fix[5 * i + k] = r[k];
+    }
+  }
+  // swing-leg and torque gains: a1_kp_foot_*, a1_kd_foot_*, a1_km_foot_* of config/<variant>_a1_<mode>.yaml (gazebo_a1_mpc.yaml:77-87,
+  // gazebo_a1_qp.yaml:34-44, hardware_a1_mpc.yaml:78-88, hardware_a1_qp.yaml:35-45, isaac_a1_mpc.yaml:78-88, isaac_a1_qp.yaml:34-44);
+  // torques_gravity (A1CtrlStates.h:129)
+  {
+    // [variant][mode QP, MPC][kp x y z, kd x y z, km x y z]
+    static const double g[3][2][9] = {{{300, 400, 400, 8, 8, 8, 0.1, 0.1, 0.1}, {200, 200, 150, 10, 10, 5, 0.1, 0.1, 0.1}},
+                                      {{260, 260, 350, 6, 6, 5, 0.1, 0.1, 0.1}, {120, 120, 80, 6, 6, 5, 0.1, 0.1, 0.1}},
+                                      {{4250, 4250, 3000, 0, 0, 0, 0.5, 0.5, 0.5}, {3250, 3250, 4000, 5, 5, 5, 0.5, 0.5, 0.5}}};
+    const double* k = g[v][mpc ? 1 : 0];
+    for (int i = 0; i < 12; ++i) { tp->kp_foot[i] = k[i % 3]; tp->kd_foot[i] = k[3 + i % 3]; }
+    for (int a = 0; a < 3; ++a) tp->km_foot[a] = k[6 + a];
+    const double tg[12] = {0.80, 0, 0, -0.80, 0, 0, 0.80, 0, 0, -0.80, 0, 0};
+    for (int i = 0; i < 12; ++i) tp->torques_gravity[i] = tg[i];
+  }
+  // the stance PD gains of the QP branch: a1_kd_linear_*, a1_kp_angular_*, a1_kd_angular_* (gazebo_a1_qp.yaml:58-68, hardware_a1_qp.yaml:59-69,
+  // isaac_a1_qp.yaml:58-68); the MPC configs set none, so MPC mode gets the ROS defaults (A1CtrlStates.h:278-296: 70, 70, 120 / 250, 35, 1 /
+  // 1.5, 1.5, 30), which the MPC branch does not read
+  {
+    static const double qp[3][9] = {{70, 70, 120, 150, 150, 1, 4.5, 4.5, 30},
+                                    {300, 200, 120, 40, 40, 10, 1, 1, 0.5},
+                                    {2600, 2600, 0, 420, 420, 150, 0, 0, 560}};
+    static const double ros[9] = {70, 70, 120, 250, 35, 1, 1.5, 1.5, 30};
+    const double* k = mpc ? ros : qp[v];
+    for (int a = 0; a < 3; ++a) { tp->kd_linear[a] = k[a]; tp->kp_angular[a] = k[3 + a]; tp->kd_angular[a] = k[6 + a]; }
+  }
+  return A1MPC_OK;
+}
+
+int a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc_tick** out) {
+  if (!h || !tp || !out) return fail(A1MPC_EINVAL, "null argument");
+  *out = nullptr;
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (h->cfg.precision != 64) return fail(A1MPC_EINVAL, "a tick needs precision 64 (its front stages are fp64)");
+  if (tp->mode != A1MPC_TICK_QP && tp->mode != A1MPC_TICK_MPC) return fail(A1MPC_EINVAL, "unknown mode");
+  const int v = tp->command.variant;
+  if (v != A1MPC_VARIANT_GAZEBO && v != A1MPC_VARIANT_HARDWARE && v != A1MPC_VARIANT_ISAAC) return fail(A1MPC_EINVAL, "unknown variant");
+  if (!(tp->gait.counter_per_swing > 0.0)) return fail(A1MPC_EINVAL, "counter_per_swing must be positive");
+  if (!(tp->command.body_height_min <= tp->command.body_height_max)) return fail(A1MPC_EINVAL, "body_height_min must not exceed body_height_max");
+  CK(cudaSetDevice(h->device));
+  const size_t lb = (size_t)B;
+  const bool mpc = tp->mode == A1MPC_TICK_MPC;
+  const bool warm = mpc && h->cfg.horizon == 10;
+  const bool filtered = v != A1MPC_VARIANT_HARDWARE;
+  auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  // [rows][B] doubles of every intermediate and state array, then the 4-byte arrays, then the warm buffer
+  const size_t nd[] = {9, 9, 12, 3, 3, 12, 12, 36, 12, 3, 12, 9, 12, 12, 4, 12, filtered ? imu_state_doubles() : 0, command_state_doubles(),
+                       (size_t)SW_FIELDS, (size_t)EKF_STATE_DOUBLES};
+  size_t bytes = 0;
+  for (size_t r : nd) bytes += pad(r * lb * sizeof(double));
+  bytes += 5 * pad(lb * 4);
+  if (warm) bytes += pad(a1mpc_warm_bytes(h, B));
+  a1mpc_tick* t = new a1mpc_tick();
+  t->h = h; t->B = B; t->tp = *tp;
+  if (cudaMalloc(&t->mem, bytes) != cudaSuccess) {
+    cudaGetLastError();
+    delete t;
+    return fail(A1MPC_ENOMEM, "cudaMalloc failed");
+  }
+  char* cur = static_cast<char*>(t->mem);
+  auto take = [&](size_t n) { char* p = n ? cur : nullptr; cur += pad(n); return p; };
+  double** dst[] = {&t->rot, &t->rz, &t->x0, &t->ia, &t->ig, &t->fpr, &t->fvr, &t->jac, &t->foot, &t->kpl, &t->des, &t->ref, &t->fk, &t->f_body,
+                    &t->gc, &t->tau, &t->imu, &t->cmd, &t->swing, &t->ekf};
+  for (size_t i = 0; i < sizeof(nd) / sizeof(nd[0]); ++i) *dst[i] = reinterpret_cast<double*>(take(nd[i] * lb * sizeof(double)));
+  t->mode = reinterpret_cast<uint32_t*>(take(lb * 4));
+  t->contact = reinterpret_cast<uint32_t*>(take(lb * 4));
+  t->est_contacts = reinterpret_cast<uint32_t*>(take(lb * 4));
+  t->status = reinterpret_cast<int32_t*>(take(lb * 4));
+  t->est_status = reinterpret_cast<int32_t*>(take(lb * 4));
+  t->warm = warm ? reinterpret_cast<uint32_t*>(take(a1mpc_warm_bytes(h, B))) : nullptr;
+  int rc;
+  if ((rc = ensure_capacity(h, B)) || (rc = ensure_lists(h, stance_scratch_bytes(B))) || (rc = tick_reset_impl(t))) {
+    a1mpc_tick_destroy(t);
+    return rc;
+  }
+  *out = t;
+  return A1MPC_OK;
+}
+
+int a1mpc_tick_reset(a1mpc_tick* t) {
+  if (!t) return fail(A1MPC_EINVAL, "null argument");
+  return tick_reset_impl(t);
+}
+
+int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out) {
+  if (!t || !in || !out || !out->tau) return fail(A1MPC_EINVAL, "null argument");
+  if (!in->quat || !in->gyro || !in->acc || !in->joint_pos || !in->joint_vel || !in->foot_force || !in->cmd || !in->gait_counter_speed)
+    return fail(A1MPC_EINVAL, "null input array");
+  if (!(dt > 0.0)) return fail(A1MPC_EINVAL, "dt must be positive");
+  const bool mpc = t->tp.mode == A1MPC_TICK_MPC;
+  if (!mpc && out->ref) return fail(A1MPC_EINVAL, "ref is an MPC-mode output: pass NULL in QP mode");
+  a1mpc_handle* h = t->h;
+  const int B = t->B;
+  const size_t lb = (size_t)B;
+  CK(cudaSetDevice(h->device));
+  const double *quat = in->quat, *gyro = in->gyro, *acc = in->acc, *jp = in->joint_pos, *jv = in->joint_vel, *ff = in->foot_force, *cmd = in->cmd,
+               *gcs = in->gait_counter_speed;
+  Stage st(h, B);
+  st.in(quat, 4); st.in(gyro, 3); st.in(acc, 3); st.in(jp, 12); st.in(jv, 12); st.in(ff, 4); st.in(cmd, 7); st.in(gcs, 4);
+  for (const void* p : {(const void*)out->tau, (const void*)out->f_body, (const void*)out->status, (const void*)out->contacts,
+                        (const void*)out->movement_mode, (const void*)out->x0, (const void*)out->ref})
+    st.unused(p);   // written by the copies at the end
+  int rc;
+  if ((rc = st.begin())) return rc;
+  if ((rc = ensure_capacity(h, B))) return rc;   // create sized the scratch and it only grows: no allocation here
+  if (!mpc && (rc = ensure_lists(h, stance_scratch_bytes(B)))) return rc;
+  const a1mpc_tick_params& tp = t->tp;
+  // 1-3: orientation and command
+  CK(tick_front_a_launch(B, dt, quat, gyro, acc, t->imu, t->rot, t->rz, t->x0, t->ia, t->ig, t->cmd, cmd, t->mode, t->kpl, mpc ? t->ref : nullptr,
+                         t->des, h->stream));
+  // 2, 4, 5: kinematics, update_plan, swing legs
+  {
+    LegParams LP;
+    for (int i = 0; i < 12; ++i) LP.rho_opt[i] = tp.rho_opt[i];
+    for (int i = 0; i < 20; ++i) LP.rho_fix[i] = tp.rho_fix[i];
+    GaitDev G;
+    G.cpg = tp.gait.counter_per_gait; G.cps = tp.gait.counter_per_swing; G.cdt = tp.gait.control_dt;
+    G.dxl = tp.gait.foot_delta_x_limit; G.dyl = tp.gait.foot_delta_y_limit;
+    for (int i = 0; i < 12; ++i) G.dfp[i] = tp.gait.default_foot_pos[i];
+    G.N = 0;
+    SwingParams SP;
+    SP.cps = tp.gait.counter_per_swing;
+    SP.dt = dt;
+    for (int i = 0; i < 12; ++i) { SP.kp[i] = tp.kp_foot[i]; SP.kd[i] = tp.kd_foot[i]; }
+    const double* lvd = mpc ? t->ref + 5 * lb : t->des + 6 * lb;
+    tick_front_b<<<(B + 127) / 128, 128, 0, h->stream>>>(B, LP, G, SP, jp, jv, t->rot, t->rz, t->x0, lvd, t->mode, t->gc, gcs, t->swing, ff, t->fpr,
+                                                         t->jac, t->fvr, t->foot, t->fk, t->contact);
+    h->launches += 2;
+    CK(cudaGetLastError());
+  }
+  // 6: EKF into x0 rows 3-5 and 9-11
+  if (t->first) {
+    ekf_init_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->ekf, t->fpr, t->rot);
+    h->launches++;
+    CK(cudaGetLastError());
+  } else if ((rc = enqueue_ekf_update(h, B, t->ekf, EkfParams{dt, tp.assume_flat_ground ? 1 : 0}, t->mode, t->ia, t->ig, t->rot, t->fpr, t->fvr, ff,
+                                      t->x0 + 3 * lb, t->x0 + 9 * lb, t->est_contacts, t->est_status))) {
+    return rc;
+  }
+  t->first = false;
+  // 7: terrain pitch and the MPC solve, or the stance QP
+  if (mpc) {
+    terrain_pitch_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->swing, tp.use_terrain_adapt ? 1 : 0, t->x0 + 3 * lb, t->ref, lb, nullptr);
+    h->launches++;
+    CK(cudaGetLastError());
+    const DevInputs di{t->x0, t->rot, t->foot, t->ref, t->contact, lb, 0};
+    const DevOutputs dout{t->f_body, t->status, nullptr, nullptr, lb, 0};
+    if ((rc = enqueue_solve(h, B, di, dout, t->warm, 0))) return rc;
+  } else {
+    double gains[9];
+    for (int i = 0; i < 3; ++i) { gains[i] = tp.kd_linear[i]; gains[3 + i] = tp.kp_angular[i]; gains[6 + i] = tp.kd_angular[i]; }
+    int nl = 0;
+    cudaError_t e = stance_qp_launch(h->sm_count, B, lb, t->x0, t->rot, t->rz, t->foot, t->contact, t->des, t->kpl, gains, h->cfg.mass, t->f_body,
+                                     t->status, nullptr, h->d_lists, h->stream, &nl);
+    if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("stance_qp kernels: ") + cudaGetErrorString(e));
+    h->launches += nl;
+  }
+  // 8: joint torques
+  {
+    TorqueParams P;
+    for (int i = 0; i < 3; ++i) P.km[i] = tp.km_foot[i];
+    for (int i = 0; i < 12; ++i) P.tg[i] = tp.torques_gravity[i];
+    joint_torques_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->f_body, t->fk, t->jac, t->contact, P, t->tau);
+    h->launches++;
+    CK(cudaGetLastError());
+  }
+  const cudaMemcpyKind kind = st.host() ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+  const struct { void* dst; const void* src; size_t bytes; } copies[] = {
+      {out->tau, t->tau, 12 * lb * 8}, {out->f_body, t->f_body, 12 * lb * 8}, {out->status, t->status, lb * 4}, {out->contacts, t->contact, lb * 4},
+      {out->movement_mode, t->mode, lb * 4}, {out->x0, t->x0, 12 * lb * 8}, {out->ref, t->ref, 9 * lb * 8}};
+  for (const auto& c : copies)
+    if (c.dst) CK(cudaMemcpyAsync(c.dst, c.src, c.bytes, kind, h->stream));
+  return st.finish();
+}
+
+int a1mpc_tick_destroy(a1mpc_tick* t) {
+  if (!t) return A1MPC_OK;
+  cudaSetDevice(t->h->device);
+  cudaStreamSynchronize(t->h->stream);
+  if (t->mem) cudaFree(t->mem);
+  delete t;
+  return A1MPC_OK;
 }
 
 // ---- helpers -------------------------------------------------------------------------------

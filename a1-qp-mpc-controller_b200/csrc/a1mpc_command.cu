@@ -1,5 +1,5 @@
-// a1mpc_command.cu -- launches of the orientation and command stages (kernels in a1mpc_command.cuh) for a1mpc_api.cu.  A translation
-// unit of their own, so that the other kernels of the library compile exactly as they did without them.
+// a1mpc_command.cu -- launches of the orientation and command stages and of the fused front of a tick (kernels in a1mpc_command.cuh) for
+// a1mpc_api.cu.  A translation unit of their own, so that the other kernels of the library compile exactly as they did without them.
 #include "a1mpc_internal.h"
 #include "a1mpc_command.cuh"
 
@@ -32,6 +32,15 @@ cudaError_t command_init_launch(int B, const a1mpc_command_params& cp, double* s
 cudaError_t command_launch(int B, double dt, double* state, const double* cmd, const double* root_pos, size_t pos_ld, uint32_t* movement_mode,
                            double* kp, double* ref, size_t ref_ld, double* des, size_t des_ld, cudaStream_t st) {
   command_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, dt, state, cmd, root_pos, pos_ld, movement_mode, kp, ref, ref_ld, des, des_ld);
+  return cudaGetLastError();
+}
+
+cudaError_t tick_front_a_launch(int B, double dt, const double* quat, const double* gyro, const double* acc, double* imu, double* rot, double* rot_z,
+                                double* x0, double* imu_acc, double* imu_ang_vel, double* cmd_state, const double* cmd, uint32_t* movement_mode,
+                                double* kp, double* ref, double* des, cudaStream_t st) {
+  const size_t lb = (size_t)B;
+  tick_front_a<<<(B + 127) / 128, 128, 0, st>>>(B, dt, quat, gyro, acc, imu, rot, rot_z, x0, x0 + 6 * lb, imu_acc, imu_ang_vel, cmd_state, cmd,
+                                                x0 + 3 * lb, movement_mode, kp, ref, des);
   return cudaGetLastError();
 }
 

@@ -45,11 +45,11 @@ __global__ void imu_init_kernel(int B, double* __restrict__ state) {
 // one IMU sample and one pose per robot, thread per robot.  quat [4][B] (w, x, y, z), gyro / acc [3][B] and imu_acc / imu_ang_vel
 // [3][B] have leading dimension B; rot, rot_z [9][B], euler and ang_vel [3][B] (rows 0-2 and 6-8 of x0) leading dimension ld.  imu
 // (the filter state), acc and every output may be null.
-__global__ void orientation_kernel(int B, const double* __restrict__ quat, const double* __restrict__ gyro, const double* __restrict__ acc,
-                                   double* __restrict__ imu, double* __restrict__ rot, double* __restrict__ rot_z, double* __restrict__ euler,
-                                   double* __restrict__ ang_vel, size_t ld, double* __restrict__ imu_acc, double* __restrict__ imu_ang_vel) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+// the per-robot body of orientation_kernel, shared with tick_front_a
+__device__ __forceinline__ void orientation_body(int b, int B, const double* __restrict__ quat, const double* __restrict__ gyro,
+                                                 const double* __restrict__ acc, double* __restrict__ imu, double* __restrict__ rot,
+                                                 double* __restrict__ rot_z, double* __restrict__ euler, double* __restrict__ ang_vel, size_t ld,
+                                                 double* __restrict__ imu_acc, double* __restrict__ imu_ang_vel) {
   const size_t lb = (size_t)B;
   double* s = imu ? imu + b : nullptr;
   // imu_callback (GazeboA1ROS.cpp:282-299, IsaacA1ROS.cpp:224-241): filter k of window 5, or the raw sample (HardwareA1ROS.cpp:273-274)
@@ -106,6 +106,14 @@ __global__ void orientation_kernel(int B, const double* __restrict__ quat, const
   }
 }
 
+__global__ void orientation_kernel(int B, const double* __restrict__ quat, const double* __restrict__ gyro, const double* __restrict__ acc,
+                                   double* __restrict__ imu, double* __restrict__ rot, double* __restrict__ rot_z, double* __restrict__ euler,
+                                   double* __restrict__ ang_vel, size_t ld, double* __restrict__ imu_acc, double* __restrict__ imu_ang_vel) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  orientation_body(b, B, quat, gyro, acc, imu, rot, rot_z, euler, ang_vel, ld, imu_acc, imu_ang_vel);
+}
+
 // the adapters' constructor values (GazeboA1ROS.cpp:60-62, GazeboA1ROS.h:130) and A1CtrlStates::reset() / resetFromROSParam()
 // (A1CtrlStates.h:35-36, 270-301); ref (may be null) gets the reset values of its nine rows.
 __global__ void command_init_kernel(int B, CommandInit P, double* __restrict__ state, double* __restrict__ ref, size_t ref_ld) {
@@ -131,11 +139,10 @@ __global__ void command_init_kernel(int B, CommandInit P, double* __restrict__ s
 // main_update's front half (GazeboA1ROS.cpp:122-188; HardwareA1ROS.cpp:104-158; IsaacA1ROS.cpp:81-137), thread per robot.
 // cmd [7][B]: velx, vely, velz, roll rate, pitch rate, yaw rate, toggle request.  root_pos [3][pos_ld]; kp [3][des_ld], des [12][des_ld]
 // (may be null), ref [9][ref_ld] (may be null: then root_euler_d[1] comes from the state).
-__global__ void command_kernel(int B, double dt, double* __restrict__ state, const double* __restrict__ cmd, const double* __restrict__ root_pos,
-                               size_t pos_ld, uint32_t* __restrict__ movement_mode, double* __restrict__ kp, double* __restrict__ ref, size_t ref_ld,
-                               double* __restrict__ des, size_t des_ld) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+// the per-robot body of command_kernel, shared with tick_front_a
+__device__ __forceinline__ void command_body(int b, int B, double dt, double* __restrict__ state, const double* __restrict__ cmd,
+                                             const double* __restrict__ root_pos, size_t pos_ld, uint32_t* __restrict__ movement_mode,
+                                             double* __restrict__ kp, double* __restrict__ ref, size_t ref_ld, double* __restrict__ des, size_t des_ld) {
   const size_t lb = (size_t)B;
   double* s = state + b;
   double c[7];
@@ -204,6 +211,29 @@ __global__ void command_kernel(int B, double dt, double* __restrict__ state, con
 #pragma unroll
     for (int i = 0; i < 12; ++i) des[i * des_ld + b] = d[i];
   }
+}
+
+__global__ void command_kernel(int B, double dt, double* __restrict__ state, const double* __restrict__ cmd, const double* __restrict__ root_pos,
+                               size_t pos_ld, uint32_t* __restrict__ movement_mode, double* __restrict__ kp, double* __restrict__ ref, size_t ref_ld,
+                               double* __restrict__ des, size_t des_ld) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  command_body(b, B, dt, state, cmd, root_pos, pos_ld, movement_mode, kp, ref, ref_ld, des, des_ld);
+}
+
+// The front of a control tick (a1mpc_tick_run), thread per robot: orientation_body then command_body, every array dense (ld = B).  The
+// command stage reads none of the orientation stage's outputs (root_pos is the previous tick's estimate), so the pair is the two
+// staged kernels back to back; this translation unit's --fmad=false keeps each stage's rounding what it is alone.
+__global__ void tick_front_a(int B, double dt, const double* __restrict__ quat, const double* __restrict__ gyro, const double* __restrict__ acc,
+                             double* __restrict__ imu, double* __restrict__ rot, double* __restrict__ rot_z, double* __restrict__ euler,
+                             double* __restrict__ ang_vel, double* __restrict__ imu_acc, double* __restrict__ imu_ang_vel,
+                             double* __restrict__ cmd_state, const double* __restrict__ cmd, const double* __restrict__ root_pos,
+                             uint32_t* __restrict__ movement_mode, double* __restrict__ kp, double* __restrict__ ref, double* __restrict__ des) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const size_t lb = (size_t)B;
+  orientation_body(b, B, quat, gyro, acc, imu, rot, rot_z, euler, ang_vel, lb, imu_acc, imu_ang_vel);
+  command_body(b, B, dt, cmd_state, cmd, root_pos, lb, movement_mode, kp, ref, lb, des, lb);
 }
 
 }  // namespace a1mpc

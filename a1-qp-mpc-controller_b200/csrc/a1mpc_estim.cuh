@@ -37,14 +37,12 @@ struct LegParams {
   double rho_fix[20];   // 4 legs x (ox, oy, d, lt, lc)
 };
 
-// thread per robot; batch-major SoA (ld = B).  Any output pointer may be null.
-__global__ void leg_kinematics_kernel(int B, const double* __restrict__ joint_pos, const double* __restrict__ joint_vel,
-                                      const double* __restrict__ rot, LegParams P, double* __restrict__ foot_pos_rel,
-                                      double* __restrict__ jac, double* __restrict__ foot_vel_rel, double* __restrict__ foot_pos_abs,
-                                      double* __restrict__ foot_vel_abs) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  const size_t ld = (size_t)B;
+// the per-robot body of leg_kinematics_kernel, shared with tick_front_b: keep_abs(k, v) also receives every foot_pos_abs element it stores
+template <class KeepAbs>
+__device__ __forceinline__ void leg_kinematics_body(int b, size_t ld, const double* __restrict__ joint_pos, const double* __restrict__ joint_vel,
+                                                    const double* __restrict__ rot, const LegParams& P, double* __restrict__ foot_pos_rel,
+                                                    double* __restrict__ jac, double* __restrict__ foot_vel_rel, double* __restrict__ foot_pos_abs,
+                                                    double* __restrict__ foot_vel_abs, KeepAbs&& keep_abs) {
   double R[9];
   if (rot) {
 #pragma unroll
@@ -81,7 +79,11 @@ __global__ void leg_kinematics_kernel(int B, const double* __restrict__ joint_po
     if (rot) {
       if (foot_pos_abs) {
 #pragma unroll
-        for (int a = 0; a < 3; ++a) foot_pos_abs[(size_t)(3 * leg + a) * ld + b] = R[3 * a] * p[0] + R[3 * a + 1] * p[1] + R[3 * a + 2] * p[2];
+        for (int a = 0; a < 3; ++a) {
+          const double v = R[3 * a] * p[0] + R[3 * a + 1] * p[1] + R[3 * a + 2] * p[2];
+          foot_pos_abs[(size_t)(3 * leg + a) * ld + b] = v;
+          keep_abs(3 * leg + a, v);
+        }
       }
       if (foot_vel_abs && joint_vel) {
 #pragma unroll
@@ -89,6 +91,16 @@ __global__ void leg_kinematics_kernel(int B, const double* __restrict__ joint_po
       }
     }
   }
+}
+
+// thread per robot; batch-major SoA (ld = B).  Any output pointer may be null.
+__global__ void leg_kinematics_kernel(int B, const double* __restrict__ joint_pos, const double* __restrict__ joint_vel,
+                                      const double* __restrict__ rot, LegParams P, double* __restrict__ foot_pos_rel,
+                                      double* __restrict__ jac, double* __restrict__ foot_vel_rel, double* __restrict__ foot_pos_abs,
+                                      double* __restrict__ foot_vel_abs) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  leg_kinematics_body(b, (size_t)B, joint_pos, joint_vel, rot, P, foot_pos_rel, jac, foot_vel_rel, foot_pos_abs, foot_vel_abs, [](int, double) {});
 }
 
 #if A1MPC_DMMA

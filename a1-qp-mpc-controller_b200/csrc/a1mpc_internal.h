@@ -61,5 +61,10 @@ cudaError_t orientation_launch(int B, const double* quat, const double* gyro, co
 cudaError_t command_init_launch(int B, const a1mpc_command_params& cp, double* state, double* ref, size_t ref_ld, cudaStream_t st);
 cudaError_t command_launch(int B, double dt, double* state, const double* cmd, const double* root_pos, size_t pos_ld, uint32_t* movement_mode,
                            double* kp, double* ref, size_t ref_ld, double* des, size_t des_ld, cudaStream_t st);
+// the fused front of a control tick (a1mpc_tick_run): both stages above in one thread per robot, every array dense (ld = B); x0 [12][B]
+// (rows 0-2 and 6-8 written, rows 3-5 read as root_pos); imu null = unfiltered; ref null in QP mode
+cudaError_t tick_front_a_launch(int B, double dt, const double* quat, const double* gyro, const double* acc, double* imu, double* rot, double* rot_z,
+                                double* x0, double* imu_acc, double* imu_ang_vel, double* cmd_state, const double* cmd, uint32_t* movement_mode,
+                                double* kp, double* ref, double* des, cudaStream_t st);
 
 }  // namespace a1mpc

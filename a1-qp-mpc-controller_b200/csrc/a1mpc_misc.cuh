@@ -228,16 +228,11 @@ __global__ void joint_torques_kernel(int B, const double* __restrict__ f_grf, co
 
 // update_plan (A1RobotControl.cpp:148-202): thread per robot, batch-major coalesced.
 struct GaitDev { double cpg, cps, cdt, dfp[12], dxl, dyl; int N; };
-__global__ void update_plan_kernel(int B, GaitDev G, double* __restrict__ gc, const double* __restrict__ gcs, const uint32_t* __restrict__ mode,
-                                   const double* __restrict__ lv, const double* __restrict__ lvd, const double* __restrict__ rz,
-                                   const double* __restrict__ rot, const double* __restrict__ pos, uint32_t* __restrict__ plan,
-                                   uint32_t* __restrict__ sched, double* __restrict__ t_rel, double* __restrict__ t_abs, double* __restrict__ t_world) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  const size_t ld = (size_t)B;
-  double c[4], sp[4];
+// update_plan's per-robot body in the pieces tick_front_b shares with update_plan_kernel.
+// The gait counters: advanced and stored, the planned contact mask returned; c and sp keep the new counters and the speeds.
+__device__ __forceinline__ uint32_t update_plan_counters(int b, size_t ld, GaitDev G, double* __restrict__ gc, const double* __restrict__ gcs, bool walk,
+                                                        double (&c)[4], double (&sp)[4]) {
   uint32_t m = 0;
-  const bool walk = mode[b] != 0;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     sp[i] = gcs[(size_t)i * ld + b];
@@ -250,6 +245,46 @@ __global__ void update_plan_kernel(int B, GaitDev G, double* __restrict__ gc, co
     }
     gc[(size_t)i * ld + b] = c[i];
   }
+  return m;
+}
+
+// what the foothold targets of the four legs share
+struct PlanTargets { double vd[3], R[9], p[3], vr0, vr1, kf; };
+__device__ __forceinline__ void plan_targets_setup(int b, size_t ld, GaitDev G, const double* __restrict__ lv, const double* __restrict__ lvd,
+                                                   const double* __restrict__ rz, const double* __restrict__ rot, const double* __restrict__ pos,
+                                                   PlanTargets& T) {
+  double v[3], Rz[9];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) { v[k] = lv[(size_t)k * ld + b]; T.vd[k] = lvd[(size_t)k * ld + b]; T.p[k] = pos[(size_t)k * ld + b]; }
+#pragma unroll
+  for (int k = 0; k < 9; ++k) { Rz[k] = rz[(size_t)k * ld + b]; T.R[k] = rot[(size_t)k * ld + b]; }
+  T.vr0 = Rz[0] * v[0] + Rz[3] * v[1] + Rz[6] * v[2];   // Rz^T v
+  T.vr1 = Rz[1] * v[0] + Rz[4] * v[1] + Rz[7] * v[2];
+  T.kf = sqrt(fabs(G.dfp[8]) / 9.8);   // default_foot_pos(2): third scalar of the 3 x 4 matrix = z of leg 0
+}
+
+// the Raibert foothold of leg i at gait counter speed sp, body frame (foot_pos_target_rel).  Its callers run it in a rolled leg loop: kf * (v - vd) is then hoisted
+// out of the loop and the other product is the one contracted into an FMA, in either kernel.
+__device__ __forceinline__ void plan_target_leg(int i, GaitDev G, double sp, const PlanTargets& T, double (&f)[3]) {
+  double dx = T.kf * (T.vr0 - T.vd[0]) + ((G.cps / sp) * G.cdt) / 2.0 * T.vd[0];
+  double dy = T.kf * (T.vr1 - T.vd[1]) + ((G.cps / sp) * G.cdt) / 2.0 * T.vd[1];
+  dx = fmin(fmax(dx, -G.dxl), G.dxl);
+  dy = fmin(fmax(dy, -G.dyl), G.dyl);
+  f[0] = G.dfp[0 * 4 + i] + dx;
+  f[1] = G.dfp[1 * 4 + i] + dy;
+  f[2] = G.dfp[2 * 4 + i];
+}
+
+__global__ void update_plan_kernel(int B, GaitDev G, double* __restrict__ gc, const double* __restrict__ gcs, const uint32_t* __restrict__ mode,
+                                   const double* __restrict__ lv, const double* __restrict__ lvd, const double* __restrict__ rz,
+                                   const double* __restrict__ rot, const double* __restrict__ pos, uint32_t* __restrict__ plan,
+                                   uint32_t* __restrict__ sched, double* __restrict__ t_rel, double* __restrict__ t_abs, double* __restrict__ t_world) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const size_t ld = (size_t)B;
+  double c[4], sp[4];
+  const bool walk = mode[b] != 0;
+  const uint32_t m = update_plan_counters(b, ld, G, gc, gcs, walk, c, sp);
   plan[b] = m;
   if (sched) {
     for (int st = 0; st < G.N; ++st) {
@@ -263,25 +298,17 @@ __global__ void update_plan_kernel(int B, GaitDev G, double* __restrict__ gc, co
     }
   }
   if (t_rel || t_abs || t_world) {
-    double v[3], vd[3], Rz[9], R[9], p[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { v[k] = lv[(size_t)k * ld + b]; vd[k] = lvd[(size_t)k * ld + b]; p[k] = pos[(size_t)k * ld + b]; }
-#pragma unroll
-    for (int k = 0; k < 9; ++k) { Rz[k] = rz[(size_t)k * ld + b]; R[k] = rot[(size_t)k * ld + b]; }
-    const double vr0 = Rz[0] * v[0] + Rz[3] * v[1] + Rz[6] * v[2], vr1 = Rz[1] * v[0] + Rz[4] * v[1] + Rz[7] * v[2];   // Rz^T v
-    const double kf = sqrt(fabs(G.dfp[8]) / 9.8);   // default_foot_pos(2): third scalar of the 3 x 4 matrix = z of leg 0
+    PlanTargets T;
+    plan_targets_setup(b, ld, G, lv, lvd, rz, rot, pos, T);
     for (int i = 0; i < 4; ++i) {
-      double dx = kf * (vr0 - vd[0]) + ((G.cps / sp[i]) * G.cdt) / 2.0 * vd[0];
-      double dy = kf * (vr1 - vd[1]) + ((G.cps / sp[i]) * G.cdt) / 2.0 * vd[1];
-      dx = fmin(fmax(dx, -G.dxl), G.dxl);
-      dy = fmin(fmax(dy, -G.dyl), G.dyl);
-      const double f[3] = {G.dfp[0 * 4 + i] + dx, G.dfp[1 * 4 + i] + dy, G.dfp[2 * 4 + i]};
+      double f[3];
+      plan_target_leg(i, G, sp[i], T, f);
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
-        const double fa = R[3 * a] * f[0] + R[3 * a + 1] * f[1] + R[3 * a + 2] * f[2];
+        const double fa = T.R[3 * a] * f[0] + T.R[3 * a + 1] * f[1] + T.R[3 * a + 2] * f[2];
         if (t_rel) t_rel[(size_t)(3 * i + a) * ld + b] = f[a];
         if (t_abs) t_abs[(size_t)(3 * i + a) * ld + b] = fa;
-        if (t_world) t_world[(size_t)(3 * i + a) * ld + b] = fa + p[a];
+        if (t_world) t_world[(size_t)(3 * i + a) * ld + b] = fa + T.p[a];
       }
     }
   }

@@ -1,0 +1,78 @@
+// a1mpc_tick.cuh -- the middle of a control tick (a1mpc_tick_run) in one kernel: leg kinematics, update_plan and generate_swing_legs_ctrl in
+// one thread per robot, from the per-robot bodies of leg_kinematics_kernel, update_plan_kernel and swing_legs_kernel.
+// Include from exactly one translation unit (a1mpc_api.cu) -- and from tests/emu (g++, A1MPC_EMU).
+//
+// What crosses a stage boundary in registers instead of memory: foot_pos_abs (kinematics -> swing), plan_contacts and foot_pos_target_rel
+// (update_plan -> swing).  Neither of the latter two is stored, and no contact schedule is computed.  The stored outputs are the ones later
+// stages read: foot_pos_rel, foot_vel_rel and jac (EKF, torques), foot_pos_abs (the solve's foot), f_kin and contacts (solve, torques), and
+// the gait counters and swing state (next tick).
+// Bit-identity with the staged kernels: the compiler contracts products into FMAs per kernel, so every stage keeps the loop shape it has
+// in its own kernel.  The foothold targets and the swing legs run in one rolled leg loop, as both do in update_plan_kernel and
+// swing_legs_kernel: unrolled, the foothold's loop-invariant product kf * (v - vd) is no longer hoisted and the other product of dx / dy gets
+// contracted, which moves the targets by an ulp.  The loop index then selects each leg's registers instead of indexing an array, which would
+// go to local memory.
+#pragma once
+#include "a1mpc_estim.cuh"
+#include "a1mpc_misc.cuh"
+#include "a1mpc_swing.cuh"
+
+namespace a1mpc {
+
+// value i of four held in registers, for an index the rolled leg loop does not know at compile time
+__device__ __forceinline__ double leg_select(double v0, double v1, double v2, double v3, int i) {
+  return i == 0 ? v0 : (i == 1 ? v1 : (i == 2 ? v2 : v3));
+}
+
+// the swing stage's inputs as tick_front_b holds them: the gait counters from memory (this thread has just written them), the planned
+// contacts, this leg's foothold target and the four feet's foot_pos_abs in registers (the leg's three selected by the loop index)
+struct SwingSrcTick {
+  const double* gc;
+  uint32_t pl;
+  const double (&fpa)[12];
+  const double (&tgt)[3];
+  size_t ld;
+  int b;
+  __device__ __forceinline__ uint32_t plan() const { return pl; }
+  __device__ __forceinline__ double g(int i) const { return gc[(size_t)i * ld + b]; }
+  __device__ __forceinline__ double p(int i, int a) const { return leg_select(fpa[a], fpa[3 + a], fpa[6 + a], fpa[9 + a], i); }
+  __device__ __forceinline__ double fin(int, int a) const { return tgt[a]; }
+};
+
+// every array dense (ld = B).  x0 [12][B]: rows 3-5 (root_pos) and 9-11 (root_lin_vel) read; lin_vel_d [3][B] is ref + 5 B (MPC mode) or
+// des + 6 B (QP mode).
+__global__ void tick_front_b(int B, LegParams LP, GaitDev G, SwingParams SP, const double* __restrict__ joint_pos, const double* __restrict__ joint_vel,
+                             const double* __restrict__ rot, const double* __restrict__ rot_z, const double* __restrict__ x0,
+                             const double* __restrict__ lin_vel_d, const uint32_t* __restrict__ mode, double* __restrict__ gc,
+                             const double* __restrict__ gcs, double* __restrict__ swing_state, const double* __restrict__ foot_force,
+                             double* __restrict__ fpr, double* __restrict__ jac, double* __restrict__ fvr, double* __restrict__ foot,
+                             double* __restrict__ fkin, uint32_t* __restrict__ contacts) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const size_t ld = (size_t)B;
+  // leg kinematics
+  double fpa[12];
+  leg_kinematics_body(b, ld, joint_pos, joint_vel, rot, LP, fpr, jac, fvr, foot, nullptr, [&](int k, double v) { fpa[k] = v; });
+  // update_plan: gait counters and planned contacts
+  double c[4], sp[4];
+  const uint32_t plan = update_plan_counters(b, ld, G, gc, gcs, mode[b] != 0, c, sp);
+  PlanTargets T;
+  plan_targets_setup(b, ld, G, x0 + 9 * ld, lin_vel_d, rot_z, rot, x0 + 3 * ld, T);
+  // swing legs (swing_legs_kernel's body), each leg right after its foothold target, in the same rolled leg loops as the staged kernels
+  double* s = swing_state + b;
+  double R[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) R[k] = rot_z[(size_t)k * ld + b];
+  uint32_t early = (uint32_t)s[(size_t)SW_EARLY * ld];
+  uint32_t cm = 0;
+#pragma unroll 1
+  for (int i = 0; i < 4; ++i) {
+    double f[3];
+    plan_target_leg(i, G, leg_select(sp[0], sp[1], sp[2], sp[3], i), T, f);
+    const SwingSrcTick src{gc, plan, fpa, f, ld, b};
+    swing_leg(i, b, ld, SP, s, R, plan, early, cm, src, foot_force, fkin, nullptr, nullptr);
+  }
+  s[(size_t)SW_EARLY * ld] = (double)early;
+  contacts[b] = cm;
+}
+
+}  // namespace a1mpc

@@ -408,6 +408,67 @@ int  a1mpc_command_init_batch(a1mpc_handle* h, int B, void* cmd_state, const a1m
 int  a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, const double* cmd, const double* root_pos, size_t root_pos_ld,
                          uint32_t* movement_mode, double* kp_linear, double* ref, size_t ref_ld, double* des, size_t stance_ld);
 
+/* ---- a whole control tick in one call: raw sensor arrays in, joint torques out ---------------------------------------------
+ * A tick object owns the controller state of B robots (IMU filters, command state, gait counters, swing state, EKF, warm-start faces,
+ * the previous torques) and every intermediate array, and runs the stages above in the order of one main_update + compute_grf +
+ * compute_joint_torques pass:
+ *   1 orientation (the IMU filters of the Gazebo and Isaac adapters; none for A1MPC_VARIANT_HARDWARE)   2 leg kinematics   3 command
+ *   4 update_plan   5 swing legs   6 EKF: a1mpc_ekf_init_batch on the first run after create or reset, the update after that
+ *   7 A1MPC_TICK_MPC: terrain pitch, then the solve of a1mpc_solve_batch_warm with shift 0 (horizon 10) or the cold a1mpc_solve_batch
+ *     (horizon 20), the contact pattern held over the horizon as compute_grf poses it; it takes part in the fused collect
+ *     (a1mpc_peer_gather_*) exactly as a1mpc_solve_batch_warm does.
+ *     A1MPC_TICK_QP: a1mpc_stance_qp_batch.
+ *   8 joint torques.
+ * The arrays connect as in a hand-built chain of those entry points: x0 rows 3-5 / 9-11 are the EKF's estimate (zero until its first
+ * update), update_plan's root_lin_vel_d is ref row 5 (MPC) or des row 6 (QP), and in MPC mode the command stage reads ref row 1 back, so
+ * the terrain pitch of one tick is what the next tick integrates on.  Stages 1-3 and 4-5 run fused, two kernels with one thread per
+ * robot; their results are bit-identical to the staged kernels.
+ *
+ * Batch-major, ld = B, either all-host or all-device arrays in one call (host: the call copies and synchronises; device: it only enqueues,
+ * allocates nothing and does not synchronise):
+ *   in:  quat [4][B] (w, x, y, z), gyro [3][B], acc [3][B], joint_pos [12][B], joint_vel [12][B], foot_force [4][B] (already filtered),
+ *        cmd [7][B] (as a1mpc_command_batch), gait_counter_speed [4][B]
+ *   out: tau [12][B] (mandatory; an entry whose new value is NaN keeps the previous one), f_body [12][B] (foot_forces_grf), status [B] (the
+ *        solve's or the stance QP's), contacts [B], movement_mode [B], x0 [12][B], ref [9][B] (MPC mode only; NULL in QP mode).  Any but tau
+ *        may be NULL.
+ * create and reset put the state where a chain starts: zero x0, gait counters and tau; a1mpc_imu_init_batch, a1mpc_command_init_batch (with
+ * ref in MPC mode), a1mpc_swing_init_batch and a1mpc_warm_reset.  create also sizes the handle's scratch for B.  Destroy a tick before its
+ * handle.  A1MPC_EINVAL: precision 32 (these stages are fp64), an unknown mode or variant, B <= 0, dt <= 0, counter_per_swing <= 0, a mix of
+ * host and device arrays, ref in QP mode. */
+#define A1MPC_TICK_QP  0   /* stance_leg_control_type 0 */
+#define A1MPC_TICK_MPC 1   /* stance_leg_control_type 1 */
+typedef struct a1mpc_tick a1mpc_tick;
+typedef struct a1mpc_tick_params {
+  int mode;                       /* A1MPC_TICK_QP | A1MPC_TICK_MPC */
+  int use_terrain_adapt;          /* MPC mode: terrain pitch written into root_euler_d[1] */
+  int assume_flat_ground;         /* the EKF's foot-height measurement */
+  a1mpc_gait_params gait;         /* horizon unused: the tick computes no schedule */
+  a1mpc_command_params command;   /* its variant also selects the IMU filters: none for A1MPC_VARIANT_HARDWARE */
+  double rho_opt[12], rho_fix[20];               /* a1mpc_leg_kinematics_batch */
+  double kp_foot[12], kd_foot[12];               /* a1mpc_swing_legs_batch */
+  double km_foot[3], torques_gravity[12];        /* a1mpc_joint_torques_batch */
+  double kd_linear[3], kp_angular[3], kd_angular[3];   /* QP mode: a1mpc_stance_qp_batch */
+} a1mpc_tick_params;
+typedef struct a1mpc_tick_inputs {
+  const double *quat, *gyro, *acc, *joint_pos, *joint_vel, *foot_force, *cmd, *gait_counter_speed;
+} a1mpc_tick_inputs;
+typedef struct a1mpc_tick_outputs {
+  double* tau;
+  double* f_body;
+  int32_t* status;
+  uint32_t* contacts;
+  uint32_t* movement_mode;
+  double* x0;
+  double* ref;
+} a1mpc_tick_outputs;
+/* the reference's launch parameters of one adapter (config/{gazebo,hardware,isaac}_a1_{qp,mpc}.yaml, A1CtrlStates.h, A1Params.h, the adapters'
+ * leg geometry); A1MPC_EINVAL for an unknown variant or mode */
+int  a1mpc_default_tick_params(int variant, int mode, a1mpc_tick_params* tp);
+int  a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc_tick** out);
+int  a1mpc_tick_reset(a1mpc_tick* t);
+int  a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out);
+int  a1mpc_tick_destroy(a1mpc_tick* t);
+
 /* ---- device memory, stream and timing helpers (so hosts need no CUDA headers) -------------- */
 int  a1mpc_device_alloc(a1mpc_handle* h, size_t bytes, void** ptr);
 int  a1mpc_device_free(a1mpc_handle* h, void* ptr);
