@@ -194,20 +194,25 @@ __global__ void __launch_bounds__(32 * Geo<NS, N>::TW) dense_solve_kernel(const 
     }
     dmax = tmax(c, dmax);
     bad = tany(c, bad);
+    if (!bad) {
+      const double cs = dmax * FSCALE * FSCALE, hs = FSCALE * FSCALE / cs;
+      for (int e = c.tid; e < NV * NV; e += G::TS) {
+        const int j = e / NV, i = e - j * NV;
+        // symmetrise like OSQP does (osqp-eigen hands over the upper triangle only)
+        const int fi = full(i), fj = full(j);
+        const double v = (fi <= fj) ? Hb[(size_t)fi * n + fj] : Hb[(size_t)fj * n + fi];
+        bad = bad || !(fabs(v) < 1e300);   // every stance entry read: NaN / Inf / huge anywhere -> numerical, zero forces
+        Hs[e] = v * hs;
+      }
+      bad = tany(c, bad);
+    }
     int st, iters = 0;
     if (bad) {
       st = A1MPC_STATUS_NUMERICAL;
       for (int i = c.tid; i < G::NPAD; i += G::TS) c.vy[i] = 0.0;
       tsync(c);
     } else {
-      const double cs = dmax * FSCALE * FSCALE, hs = FSCALE * FSCALE / cs, gsc = FSCALE / cs;
-      for (int e = c.tid; e < NV * NV; e += G::TS) {
-        const int j = e / NV, i = e - j * NV;
-        // symmetrise like OSQP does (osqp-eigen hands over the upper triangle only)
-        const int fi = full(i), fj = full(j);
-        const double v = (fi <= fj) ? Hb[(size_t)fi * n + fj] : Hb[(size_t)fj * n + fi];
-        Hs[e] = v * hs;
-      }
+      const double gsc = FSCALE / (dmax * FSCALE * FSCALE);
       for (int v = c.tid; v < NV; v += G::TS) c.g[v] = gb[full(v)] * gsc;
       tsync(c);
       if (c.wit == 0) fill_padding<NS, N, 0>(c);

@@ -205,7 +205,13 @@ int  a1mpc_qp_rollout_batch(a1mpc_handle* h, int B, const double* A_d, const dou
 /* OsqpEigen::Solver replacement for the MPC QP (A1RobotControl.cpp:522-555):
  *   min 1/2 u'Hu + g'u  s.t. the friction pyramid of ConvexMpc.cpp:46-58 with the contact
  *   pattern `contact` (constant over the horizon).  H [B][12N][12N], g [B][12N] QP-major,
- *   u [B][12N] out (getSolution()), status [B]. */
+ *   u [B][12N] out (getSolution()), status [B].
+ *   Only the upper triangle of H is read (as OSQP takes it), and only the rows and columns of the
+ *   stance feet: the strict lower triangle and the swing rows, columns and gradient entries may
+ *   hold anything.  A stance entry of H or g that is NaN, Inf or of magnitude >= 1e300, or a stance
+ *   diagonal entry <= 0, gives NUMERICAL with u all zero.  No stance foot: NO_CONTACT, u zero.
+ *   N = 10 serves every stance count; N = 20 one or two feet, while three or four end NUMERICAL
+ *   with u zero (their dense factor does not fit in shared memory). */
 int  a1mpc_solve_dense_batch(a1mpc_handle* h, int B, const double* H, const double* g,
                              const uint32_t* contact, double* u, int32_t* status);
 
