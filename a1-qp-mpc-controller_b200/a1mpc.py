@@ -279,7 +279,11 @@ class DeviceBatch:
 
 
 class Tick:
-    """a whole control tick for B robots (a1mpc_tick_*): owns the controller state; raw sensor arrays in, joint torques out"""
+    """a whole control tick for B robots (a1mpc_tick_*): owns the controller state; raw sensor arrays in, joint torques out.
+
+    In MPC mode params.gait.horizon picks how the solve is posed: 0 (the default) holds the current contact pattern over the horizon as
+    the reference does; the engine's horizon runs the scheduled tick, whose solve sees the gait's planned contacts over the horizon (step 0
+    the swing stage's contacts) and does not take part in the fused collect.  Any other value is rejected; QP mode ignores it."""
 
     _SHAPES = dict(quat=(4,), gyro=(3,), acc=(3,), joint_pos=(12,), joint_vel=(12,), foot_force=(4,), cmd=(7,), gait_counter_speed=(4,))
 

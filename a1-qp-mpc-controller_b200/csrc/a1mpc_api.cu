@@ -116,6 +116,18 @@ int ensure_side(a1mpc_handle* h, size_t bytes) {
   return A1MPC_OK;
 }
 
+// the extended path's record queues (the general kernel's, then the compacted class's) for h->cap QPs; call after ensure_capacity
+int ensure_capacity_ext(a1mpc_handle* h, size_t B) {
+  if (B > h->cap_ext) {
+    CK(cudaStreamSynchronize(h->stream));
+    if (h->d_rec_ext) cudaFree(h->d_rec_ext);
+    h->d_rec_ext = nullptr;
+    CK(cudaMalloc(&h->d_rec_ext, 2 * h->cap * REC_EXT_BYTES));   // second half: queue of the compacted class
+    h->cap_ext = h->cap;
+  }
+  return A1MPC_OK;
+}
+
 int ensure_lists(a1mpc_handle* h, size_t bytes) {
   if (bytes > h->lists_bytes) {
     CK(cudaStreamSynchronize(h->stream));
@@ -293,13 +305,8 @@ int enqueue_solve(a1mpc_handle* h, int B, const DevInputs& din, const DevOutputs
 int enqueue_solve_ext(a1mpc_handle* h, int B, const DevInputs& di, const uint32_t* dsched, const double* dnorm, const DevOutputs& dout_in,
                       uint32_t* warm, int shift) {
   const int N = h->cfg.horizon;
-  if ((size_t)B > h->cap_ext) {
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->d_rec_ext) cudaFree(h->d_rec_ext);
-    h->d_rec_ext = nullptr;
-    CK(cudaMalloc(&h->d_rec_ext, 2 * h->cap * REC_EXT_BYTES));   // second half: queue of the compacted class
-    h->cap_ext = h->cap;
-  }
+  int rc;
+  if ((rc = ensure_capacity_ext(h, B))) return rc;
   DevOutputs dout = dout_in;
   attach_peers(h, -1, dout);   // the fused collect is wired to a1mpc_solve_batch / _warm only
 #if A1MPC_TIMELINE
@@ -937,6 +944,7 @@ struct a1mpc_tick {
   // intermediates, dense [rows][B]
   double *rot, *rz, *x0, *ia, *ig, *fpr, *fvr, *jac, *foot, *kpl, *des, *ref, *fk, *f_body;
   uint32_t *mode, *contact, *est_contacts;
+  uint32_t* sched;        // the scheduled tick's contact schedule [N][B] (gait.horizon = N), else NULL
   int32_t *status, *est_status;
   // state
   double *gc, *tau, *imu, *cmd, *swing, *ekf;
@@ -1065,18 +1073,22 @@ int a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc
   if (v != A1MPC_VARIANT_GAZEBO && v != A1MPC_VARIANT_HARDWARE && v != A1MPC_VARIANT_ISAAC) return fail(A1MPC_EINVAL, "unknown variant");
   if (!(tp->gait.counter_per_swing > 0.0)) return fail(A1MPC_EINVAL, "counter_per_swing must be positive");
   if (!(tp->command.body_height_min <= tp->command.body_height_max)) return fail(A1MPC_EINVAL, "body_height_min must not exceed body_height_max");
+  const bool mpc = tp->mode == A1MPC_TICK_MPC;
+  if (mpc && tp->gait.horizon != 0 && tp->gait.horizon != h->cfg.horizon)
+    return fail(A1MPC_EINVAL, "gait.horizon must be 0 (the held contact pattern) or the handle's horizon (the scheduled tick)");
+  const bool sched = mpc && tp->gait.horizon != 0;
   CK(cudaSetDevice(h->device));
   const size_t lb = (size_t)B;
-  const bool mpc = tp->mode == A1MPC_TICK_MPC;
   const bool warm = mpc && h->cfg.horizon == 10;
   const bool filtered = v != A1MPC_VARIANT_HARDWARE;
   auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  // [rows][B] doubles of every intermediate and state array, then the 4-byte arrays, then the warm buffer
+  // [rows][B] doubles of every intermediate and state array, then the 4-byte arrays, the schedule and the warm buffer
   const size_t nd[] = {9, 9, 12, 3, 3, 12, 12, 36, 12, 3, 12, 9, 12, 12, 4, 12, filtered ? imu_state_doubles() : 0, command_state_doubles(),
                        (size_t)SW_FIELDS, (size_t)EKF_STATE_DOUBLES};
   size_t bytes = 0;
   for (size_t r : nd) bytes += pad(r * lb * sizeof(double));
   bytes += 5 * pad(lb * 4);
+  if (sched) bytes += pad((size_t)h->cfg.horizon * lb * 4);
   if (warm) bytes += pad(a1mpc_warm_bytes(h, B));
   a1mpc_tick* t = new a1mpc_tick();
   t->h = h; t->B = B; t->tp = *tp;
@@ -1095,9 +1107,12 @@ int a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc
   t->est_contacts = reinterpret_cast<uint32_t*>(take(lb * 4));
   t->status = reinterpret_cast<int32_t*>(take(lb * 4));
   t->est_status = reinterpret_cast<int32_t*>(take(lb * 4));
+  t->sched = sched ? reinterpret_cast<uint32_t*>(take((size_t)h->cfg.horizon * lb * 4)) : nullptr;
   t->warm = warm ? reinterpret_cast<uint32_t*>(take(a1mpc_warm_bytes(h, B))) : nullptr;
   int rc;
-  if ((rc = ensure_capacity(h, B)) || (rc = ensure_lists(h, stance_scratch_bytes(B))) || (rc = tick_reset_impl(t))) {
+  // the scheduled solve's record queues too, so that a run allocates nothing
+  if ((rc = ensure_capacity(h, B)) || (sched && (rc = ensure_capacity_ext(h, B))) || (rc = ensure_lists(h, stance_scratch_bytes(B))) ||
+      (rc = tick_reset_impl(t))) {
     a1mpc_tick_destroy(t);
     return rc;
   }
@@ -1132,11 +1147,12 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
   if ((rc = st.begin())) return rc;
   if ((rc = ensure_capacity(h, B))) return rc;   // create sized the scratch and it only grows: no allocation here
   if (!mpc && (rc = ensure_lists(h, stance_scratch_bytes(B)))) return rc;
+  if (t->sched && (rc = ensure_capacity_ext(h, B))) return rc;
   const a1mpc_tick_params& tp = t->tp;
   // 1-3: orientation and command
   CK(tick_front_a_launch(B, dt, quat, gyro, acc, t->imu, t->rot, t->rz, t->x0, t->ia, t->ig, t->cmd, cmd, t->mode, t->kpl, mpc ? t->ref : nullptr,
                          t->des, h->stream));
-  // 2, 4, 5: kinematics, update_plan, swing legs
+  // 2, 4, 5: kinematics, update_plan, swing legs; the scheduled tick also writes the schedule
   {
     LegParams LP;
     for (int i = 0; i < 12; ++i) LP.rho_opt[i] = tp.rho_opt[i];
@@ -1145,14 +1161,18 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
     G.cpg = tp.gait.counter_per_gait; G.cps = tp.gait.counter_per_swing; G.cdt = tp.gait.control_dt;
     G.dxl = tp.gait.foot_delta_x_limit; G.dyl = tp.gait.foot_delta_y_limit;
     for (int i = 0; i < 12; ++i) G.dfp[i] = tp.gait.default_foot_pos[i];
-    G.N = 0;
+    G.N = t->sched ? h->cfg.horizon : 0;
     SwingParams SP;
     SP.cps = tp.gait.counter_per_swing;
     SP.dt = dt;
     for (int i = 0; i < 12; ++i) { SP.kp[i] = tp.kp_foot[i]; SP.kd[i] = tp.kd_foot[i]; }
     const double* lvd = mpc ? t->ref + 5 * lb : t->des + 6 * lb;
-    tick_front_b<<<(B + 127) / 128, 128, 0, h->stream>>>(B, LP, G, SP, jp, jv, t->rot, t->rz, t->x0, lvd, t->mode, t->gc, gcs, t->swing, ff, t->fpr,
-                                                         t->jac, t->fvr, t->foot, t->fk, t->contact);
+    if (t->sched)
+      tick_front_sched<<<(B + 127) / 128, 128, 0, h->stream>>>(B, LP, G, SP, jp, jv, t->rot, t->rz, t->x0, lvd, t->mode, t->gc, gcs, t->swing, ff,
+                                                               t->fpr, t->jac, t->fvr, t->foot, t->fk, t->contact, t->sched);
+    else
+      tick_front_b<<<(B + 127) / 128, 128, 0, h->stream>>>(B, LP, G, SP, jp, jv, t->rot, t->rz, t->x0, lvd, t->mode, t->gc, gcs, t->swing, ff, t->fpr,
+                                                           t->jac, t->fvr, t->foot, t->fk, t->contact);
     h->launches += 2;
     CK(cudaGetLastError());
   }
@@ -1173,7 +1193,9 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
     CK(cudaGetLastError());
     const DevInputs di{t->x0, t->rot, t->foot, t->ref, t->contact, lb, 0};
     const DevOutputs dout{t->f_body, t->status, nullptr, nullptr, lb, 0};
-    if ((rc = enqueue_solve(h, B, di, dout, t->warm, 0))) return rc;
+    // held pattern: a1mpc_solve_batch_warm, shift 0 (cold at horizon 20).  Scheduled: a1mpc_solve_batch_ext_warm on the schedule with
+    // world-z pyramids, shift 1 as the schedule moves one step per tick (a1mpc_solve_batch_ext at horizon 20, where t->warm is NULL)
+    if ((rc = t->sched ? enqueue_solve_ext(h, B, di, t->sched, nullptr, dout, t->warm, 1) : enqueue_solve(h, B, di, dout, t->warm, 0))) return rc;
   } else {
     double gains[9];
     for (int i = 0; i < 3; ++i) { gains[i] = tp.kd_linear[i]; gains[3 + i] = tp.kp_angular[i]; gains[6 + i] = tp.kd_angular[i]; }

@@ -228,7 +228,7 @@ __global__ void joint_torques_kernel(int B, const double* __restrict__ f_grf, co
 
 // update_plan (A1RobotControl.cpp:148-202): thread per robot, batch-major coalesced.
 struct GaitDev { double cpg, cps, cdt, dfp[12], dxl, dyl; int N; };
-// update_plan's per-robot body in the pieces tick_front_b shares with update_plan_kernel.
+// update_plan's per-robot body in the pieces tick_front_b and tick_front_sched share with update_plan_kernel.
 // The gait counters: advanced and stored, the planned contact mask returned; c and sp keep the new counters and the speeds.
 __device__ __forceinline__ uint32_t update_plan_counters(int b, size_t ld, GaitDev G, double* __restrict__ gc, const double* __restrict__ gcs, bool walk,
                                                         double (&c)[4], double (&sp)[4]) {
@@ -246,6 +246,22 @@ __device__ __forceinline__ uint32_t update_plan_counters(int b, size_t ld, GaitD
     gc[(size_t)i * ld + b] = c[i];
   }
   return m;
+}
+
+// The contact schedule, rows first .. N-1 of sched [N][B]: step st is the planned mask st plan ticks ahead of the counters c just
+// advanced (speeds sp); standstill plans every foot in contact at every step.  update_plan_kernel writes every row; tick_front_sched
+// writes row 0 itself, with the swing stage's contacts.
+__device__ __forceinline__ void update_plan_sched(int b, size_t ld, GaitDev G, bool walk, const double (&c)[4], const double (&sp)[4], int first,
+                                                  uint32_t* __restrict__ sched) {
+  for (int st = first; st < G.N; ++st) {
+    uint32_t ms = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const double ci = walk ? fmod(c[i] + (double)st * sp[i], G.cpg) : 0.0;
+      if (!walk || ci <= G.cps) ms |= 1u << i;
+    }
+    sched[(size_t)st * ld + b] = ms;
+  }
 }
 
 // what the foothold targets of the four legs share
@@ -286,17 +302,7 @@ __global__ void update_plan_kernel(int B, GaitDev G, double* __restrict__ gc, co
   const bool walk = mode[b] != 0;
   const uint32_t m = update_plan_counters(b, ld, G, gc, gcs, walk, c, sp);
   plan[b] = m;
-  if (sched) {
-    for (int st = 0; st < G.N; ++st) {
-      uint32_t ms = 0;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const double ci = walk ? fmod(c[i] + (double)st * sp[i], G.cpg) : 0.0;
-        if (!walk || ci <= G.cps) ms |= 1u << i;
-      }
-      sched[(size_t)st * ld + b] = ms;
-    }
-  }
+  if (sched) update_plan_sched(b, ld, G, walk, c, sp, 0, sched);
   if (t_rel || t_abs || t_world) {
     PlanTargets T;
     plan_targets_setup(b, ld, G, lv, lvd, rz, rot, pos, T);

@@ -1,9 +1,11 @@
-// a1mpc_tick.cuh -- the middle of a control tick (a1mpc_tick_run) in one kernel: leg kinematics, update_plan and generate_swing_legs_ctrl in
-// one thread per robot, from the per-robot bodies of leg_kinematics_kernel, update_plan_kernel and swing_legs_kernel.
+// a1mpc_tick.cuh -- the middle of a control tick (a1mpc_tick_run) in one kernel (tick_front_b, or tick_front_sched in the scheduled tick):
+// leg kinematics, update_plan and generate_swing_legs_ctrl in one thread per robot, from the per-robot bodies of leg_kinematics_kernel,
+// update_plan_kernel and swing_legs_kernel.
 // Include from exactly one translation unit (a1mpc_api.cu) -- and from tests/emu (g++, A1MPC_EMU).
 //
 // What crosses a stage boundary in registers instead of memory: foot_pos_abs (kinematics -> swing), plan_contacts and foot_pos_target_rel
-// (update_plan -> swing).  Neither of the latter two is stored, and no contact schedule is computed.  The stored outputs are the ones later
+// (update_plan -> swing).  Neither of the latter two is stored.  tick_front_b computes no contact schedule; tick_front_sched, the same body,
+// also writes the schedule of the scheduled tick.  The stored outputs are the ones later
 // stages read: foot_pos_rel, foot_vel_rel and jac (EKF, torques), foot_pos_abs (the solve's foot), f_kin and contacts (solve, torques), and
 // the gait counters and swing state (next tick).
 // Bit-identity with the staged kernels: the compiler contracts products into FMAs per kernel, so every stage keeps the loop shape it has
@@ -38,23 +40,26 @@ struct SwingSrcTick {
   __device__ __forceinline__ double fin(int, int a) const { return tgt[a]; }
 };
 
-// every array dense (ld = B).  x0 [12][B]: rows 3-5 (root_pos) and 9-11 (root_lin_vel) read; lin_vel_d [3][B] is ref + 5 B (MPC mode) or
-// des + 6 B (QP mode).
-__global__ void tick_front_b(int B, LegParams LP, GaitDev G, SwingParams SP, const double* __restrict__ joint_pos, const double* __restrict__ joint_vel,
-                             const double* __restrict__ rot, const double* __restrict__ rot_z, const double* __restrict__ x0,
-                             const double* __restrict__ lin_vel_d, const uint32_t* __restrict__ mode, double* __restrict__ gc,
-                             const double* __restrict__ gcs, double* __restrict__ swing_state, const double* __restrict__ foot_force,
-                             double* __restrict__ fpr, double* __restrict__ jac, double* __restrict__ fvr, double* __restrict__ foot,
-                             double* __restrict__ fkin, uint32_t* __restrict__ contacts) {
+// the body of both kernels below; sched == nullptr (tick_front_b) computes no schedule.  every array dense (ld = B).  x0 [12][B]: rows 3-5
+// (root_pos) and 9-11 (root_lin_vel) read; lin_vel_d [3][B] is ref + 5 B (MPC mode) or des + 6 B (QP mode).
+__device__ __forceinline__ void tick_front_b_body(int B, const LegParams& LP, const GaitDev& G, const SwingParams& SP, const double* __restrict__ joint_pos,
+                                                  const double* __restrict__ joint_vel, const double* __restrict__ rot, const double* __restrict__ rot_z,
+                                                  const double* __restrict__ x0, const double* __restrict__ lin_vel_d, const uint32_t* __restrict__ mode,
+                                                  double* __restrict__ gc, const double* __restrict__ gcs, double* __restrict__ swing_state,
+                                                  const double* __restrict__ foot_force, double* __restrict__ fpr, double* __restrict__ jac,
+                                                  double* __restrict__ fvr, double* __restrict__ foot, double* __restrict__ fkin,
+                                                  uint32_t* __restrict__ contacts, uint32_t* __restrict__ sched) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const size_t ld = (size_t)B;
   // leg kinematics
   double fpa[12];
   leg_kinematics_body(b, ld, joint_pos, joint_vel, rot, LP, fpr, jac, fvr, foot, nullptr, [&](int k, double v) { fpa[k] = v; });
-  // update_plan: gait counters and planned contacts
+  // update_plan: gait counters and planned contacts; schedule rows 1 .. N-1 (row 0 waits for the swing stage's contacts)
   double c[4], sp[4];
-  const uint32_t plan = update_plan_counters(b, ld, G, gc, gcs, mode[b] != 0, c, sp);
+  const bool walk = mode[b] != 0;
+  const uint32_t plan = update_plan_counters(b, ld, G, gc, gcs, walk, c, sp);
+  if (sched) update_plan_sched(b, ld, G, walk, c, sp, 1, sched);
   PlanTargets T;
   plan_targets_setup(b, ld, G, x0 + 9 * ld, lin_vel_d, rot_z, rot, x0 + 3 * ld, T);
   // swing legs (swing_legs_kernel's body), each leg right after its foothold target, in the same rolled leg loops as the staged kernels
@@ -73,6 +78,31 @@ __global__ void tick_front_b(int B, LegParams LP, GaitDev G, SwingParams SP, con
   }
   s[(size_t)SW_EARLY * ld] = (double)early;
   contacts[b] = cm;
+  if (sched) sched[b] = cm;
+}
+
+// the held-pattern tick (gait.horizon = 0): no schedule
+__global__ void tick_front_b(int B, LegParams LP, GaitDev G, SwingParams SP, const double* __restrict__ joint_pos, const double* __restrict__ joint_vel,
+                             const double* __restrict__ rot, const double* __restrict__ rot_z, const double* __restrict__ x0,
+                             const double* __restrict__ lin_vel_d, const uint32_t* __restrict__ mode, double* __restrict__ gc,
+                             const double* __restrict__ gcs, double* __restrict__ swing_state, const double* __restrict__ foot_force,
+                             double* __restrict__ fpr, double* __restrict__ jac, double* __restrict__ fvr, double* __restrict__ foot,
+                             double* __restrict__ fkin, uint32_t* __restrict__ contacts) {
+  tick_front_b_body(B, LP, G, SP, joint_pos, joint_vel, rot, rot_z, x0, lin_vel_d, mode, gc, gcs, swing_state, foot_force, fpr, jac, fvr, foot, fkin,
+                    contacts, nullptr);
+}
+
+// the scheduled tick (gait.horizon = N = G.N): tick_front_b plus the contact schedule sched [N][B] the solve takes.  Rows 1 .. N-1 are
+// update_plan's; row 0 is the swing stage's contacts (plan OR early contact), so the solve's first step stands on the feet the torque stage
+// treats as stance.
+__global__ void tick_front_sched(int B, LegParams LP, GaitDev G, SwingParams SP, const double* __restrict__ joint_pos, const double* __restrict__ joint_vel,
+                                 const double* __restrict__ rot, const double* __restrict__ rot_z, const double* __restrict__ x0,
+                                 const double* __restrict__ lin_vel_d, const uint32_t* __restrict__ mode, double* __restrict__ gc,
+                                 const double* __restrict__ gcs, double* __restrict__ swing_state, const double* __restrict__ foot_force,
+                                 double* __restrict__ fpr, double* __restrict__ jac, double* __restrict__ fvr, double* __restrict__ foot,
+                                 double* __restrict__ fkin, uint32_t* __restrict__ contacts, uint32_t* __restrict__ sched) {
+  tick_front_b_body(B, LP, G, SP, joint_pos, joint_vel, rot, rot_z, x0, lin_vel_d, mode, gc, gcs, swing_state, foot_force, fpr, jac, fvr, foot, fkin,
+                    contacts, sched);
 }
 
 }  // namespace a1mpc

@@ -420,9 +420,15 @@ int  a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, con
  * compute_joint_torques pass:
  *   1 orientation (the IMU filters of the Gazebo and Isaac adapters; none for A1MPC_VARIANT_HARDWARE)   2 leg kinematics   3 command
  *   4 update_plan   5 swing legs   6 EKF: a1mpc_ekf_init_batch on the first run after create or reset, the update after that
- *   7 A1MPC_TICK_MPC: terrain pitch, then the solve of a1mpc_solve_batch_warm with shift 0 (horizon 10) or the cold a1mpc_solve_batch
- *     (horizon 20), the contact pattern held over the horizon as compute_grf poses it; it takes part in the fused collect
- *     (a1mpc_peer_gather_*) exactly as a1mpc_solve_batch_warm does.
+ *   7 A1MPC_TICK_MPC: terrain pitch, then the MPC solve, posed one of two ways by gait.horizon:
+ *     0 (the default): the contact pattern held over the horizon as compute_grf poses it: the solve of a1mpc_solve_batch_warm with
+ *       shift 0 (horizon 10) or the cold a1mpc_solve_batch (horizon 20).  It takes part in the fused collect (a1mpc_peer_gather_*) exactly
+ *       as a1mpc_solve_batch_warm does.
+ *     the handle's horizon N: the scheduled tick, an extension beyond the reference.  The solve sees the gait's planned contacts over the
+ *       horizon: the solve of a1mpc_solve_batch_ext_warm with shift 1 (horizon 10) or the cold a1mpc_solve_batch_ext (horizon 20) on the
+ *       schedule [N][B] of a1mpc_update_plan_batch, whose step 0 is replaced by the swing stage's contacts (plan OR early contact: the
+ *       feet the torque stage treats as stance), world-z friction pyramids (no normals).  Like a1mpc_solve_batch_ext it does not take
+ *       part in the fused collect.  The schedule stays inside the tick.
  *     A1MPC_TICK_QP: a1mpc_stance_qp_batch.
  *   8 joint torques.
  * The arrays connect as in a hand-built chain of those entry points: x0 rows 3-5 / 9-11 are the EKF's estimate (zero until its first
@@ -438,9 +444,10 @@ int  a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, con
  *        solve's or the stance QP's), contacts [B], movement_mode [B], x0 [12][B], ref [9][B] (MPC mode only; NULL in QP mode).  Any but tau
  *        may be NULL.
  * create and reset put the state where a chain starts: zero x0, gait counters and tau; a1mpc_imu_init_batch, a1mpc_command_init_batch (with
- * ref in MPC mode), a1mpc_swing_init_batch and a1mpc_warm_reset.  create also sizes the handle's scratch for B.  Destroy a tick before its
- * handle.  A1MPC_EINVAL: precision 32 (these stages are fp64), an unknown mode or variant, B <= 0, dt <= 0, counter_per_swing <= 0, a mix of
- * host and device arrays, ref in QP mode. */
+ * ref in MPC mode), a1mpc_swing_init_batch and a1mpc_warm_reset.  create also sizes the handle's scratch for B (the scheduled tick's
+ * too).  Destroy a tick before its handle.  A1MPC_EINVAL: precision 32 (these stages are fp64), an unknown mode or variant, in MPC mode a
+ * gait.horizon other than 0 or the handle's horizon, B <= 0, dt <= 0, counter_per_swing <= 0, a mix of host and device arrays, ref in QP
+ * mode. */
 #define A1MPC_TICK_QP  0   /* stance_leg_control_type 0 */
 #define A1MPC_TICK_MPC 1   /* stance_leg_control_type 1 */
 typedef struct a1mpc_tick a1mpc_tick;
@@ -448,7 +455,7 @@ typedef struct a1mpc_tick_params {
   int mode;                       /* A1MPC_TICK_QP | A1MPC_TICK_MPC */
   int use_terrain_adapt;          /* MPC mode: terrain pitch written into root_euler_d[1] */
   int assume_flat_ground;         /* the EKF's foot-height measurement */
-  a1mpc_gait_params gait;         /* horizon unused: the tick computes no schedule */
+  a1mpc_gait_params gait;         /* MPC mode: horizon 0 = the held pattern, N = the handle's horizon = the scheduled tick; QP mode: unused */
   a1mpc_command_params command;   /* its variant also selects the IMU filters: none for A1MPC_VARIANT_HARDWARE */
   double rho_opt[12], rho_fix[20];               /* a1mpc_leg_kinematics_batch */
   double kp_foot[12], kd_foot[12];               /* a1mpc_swing_legs_batch */

@@ -1,6 +1,6 @@
 """dev tool: device time of one MPC-mode control tick, a1mpc_tick_run against the same stages called one by one, on device pointers.
 
-  python tools/tick_bench.py [--sizes 1024,16384,65536] [--repeats 5] [--ticks 20] [--json PATH]
+  python tools/tick_bench.py [--sizes 1024,16384,65536] [--repeats 5] [--ticks 20] [--json PATH] [--sched]
 
 For each batch size, with the card's name and power limit read (nvidia-smi, read-only query) in the same run:
   (a) the staged chain: orientation -> leg kinematics -> command -> update_plan -> swing legs -> EKF update -> terrain pitch -> warm solve
@@ -14,6 +14,9 @@ For each batch size, with the card's name and power limit read (nvidia-smi, read
   (e) the device time of the kernels, memsets and copies of (a) and of (b) per stage, per tick, from torch.profiler's CUDA activity trace
       of `ticks` ticks (a run of its own: the profiler slows the host).
 (a) and (b) report the median, min and max over the repeats of each window's mean tick time.
+With --sched the run times the scheduled tick instead (gait.horizon = the handle's horizon: the solve on update_plan's schedule with step 0
+the swing stage's contacts, a1mpc_solve_batch_ext_warm with shift 1) against the held-pattern tick (gait.horizon = 0), two a1mpc.Tick
+objects on the same inputs, alternating windows as in (a) / (b), and (e) for both.
 Inputs: tests/tick_scenarios.py, with every robot walking from tick 5 to tick `ticks` - 5 of each window, so that every window of
 `ticks` ticks does the same work.  Not part of bench.py's contract."""
 import argparse
@@ -47,7 +50,7 @@ def stats(ms):
 
 STAGES = ("orientation", "kinematics", "command", "update_plan", "swing", "ekf", "terrain", "solve", "torques")
 # kernel name -> stage of (e); every other kernel and memset of a tick belongs to the solve (pack_kernel, the class kernels)
-KERNEL_STAGE = (("tick_front_a", "front_a"), ("tick_front_b", "front_b"), ("orientation_kernel", "orientation"), ("leg_kinematics", "kinematics"),
+KERNEL_STAGE = (("tick_front_a", "front_a"), ("tick_front_b", "front_b"), ("tick_front_sched", "front_b"), ("orientation_kernel", "orientation"), ("leg_kinematics", "kinematics"),
                 ("command_kernel", "command"), ("update_plan", "update_plan"), ("swing_legs", "swing"), ("ekf_", "ekf"), ("terrain_pitch", "terrain"),
                 ("joint_torques", "torques"), ("Memcpy", "copies"))
 
@@ -76,17 +79,70 @@ def kernel_ms(eng, fn, k):
     return out
 
 
+def window_inputs(eng, B, T):
+    """tests/tick_scenarios.py's inputs with one period per window: every robot starts walking at tick 5 and stops at tick T - 5"""
+    seqs, speed = tick_inputs(B, T, B)
+    seqs["cmd"][:, 6] = 0.0
+    seqs["cmd"][5, 6] = 1.0
+    seqs["cmd"][T - 5, 6] = 1.0
+    return DeviceSeqs(a1mpc, eng, seqs, speed)
+
+
+def timed(eng, fn, k):
+    """mean device ms per call of k back-to-back calls of fn, between two CUDA events"""
+    e0, e1 = eng.event(), eng.event()
+    eng.record(e0)
+    for _ in range(k):
+        fn()
+    eng.record(e1)
+    ms = eng.elapsed_ms(e0, e1) / k
+    for e in (e0, e1):
+        a1mpc.lib().a1mpc_event_destroy(eng.h, e)
+    return ms
+
+
+def bench_sched(eng, B, repeats, ticks):
+    """--sched: the held-pattern tick against the scheduled tick, same inputs, alternating windows of `ticks` ticks"""
+    T = ticks
+    ds = window_inputs(eng, B, T)
+    tins = [a1mpc.TickInputs(*[(ds.speed if k == "gait_counter_speed" else ds.at(k, t)) for k in a1mpc.TICK_INPUTS]) for t in range(T)]
+    dtau = eng.dalloc(12 * B * 8)
+    touts = a1mpc.TickOutputs(dtau, None, None, None, None, None, None)
+    runs = {}
+    for name, horizon in (("held", 0), ("sched", eng.cfg.horizon)):
+        tp = a1mpc.default_tick_params(a1mpc.VARIANT_GAZEBO, a1mpc.TICK_MPC)
+        tp.gait.horizon = horizon
+        tick, n = a1mpc.Tick(eng, B, tp), [0]
+
+        def run(tick=tick, n=n):
+            t = n[0] % T
+            n[0] += 1
+            tick.run_ptrs(DT, tins[t], touts)
+        runs[name] = (tick, run)
+    for _ in range(T):   # warm-up: every shape of the timed window, the warm faces settled
+        for _, run in runs.values():
+            run()
+    eng.sync()
+    ms = {name: [] for name in runs}
+    for _ in range(repeats):
+        for name, (_, run) in runs.items():
+            ms[name].append(timed(eng, run, T))
+    kern = {name: kernel_ms(eng, run, T) for name, (_, run) in runs.items()}
+    eng.sync()
+    for tick, _ in runs.values():
+        tick.close()
+    a1mpc.lib().a1mpc_device_free(eng.h, dtau)
+    ds.free()
+    return dict(B=B, held=stats(ms["held"]), sched=stats(ms["sched"]), kernel_ms_per_tick=kern)
+
+
 def bench_size(eng, B, repeats, ticks):
     L = a1mpc.lib()
     T = ticks
     tp = a1mpc.default_tick_params(a1mpc.VARIANT_GAZEBO, a1mpc.TICK_MPC)
-    seqs, speed = tick_inputs(B, T, B)
-    # one period per window: every robot starts walking at tick 5 and stops at tick T - 5, so each window of T ticks starts from
-    # standstill and does the same work (the solve's cost depends strongly on the stance mix: standstill is all four-stance)
-    seqs["cmd"][:, 6] = 0.0
-    seqs["cmd"][5, 6] = 1.0
-    seqs["cmd"][T - 5, 6] = 1.0
-    ds = DeviceSeqs(a1mpc, eng, seqs, speed)
+    # one period per window, so each window of T ticks starts from standstill and does the same work (the solve's cost depends strongly
+    # on the stance mix: standstill is all four-stance)
+    ds = window_inputs(eng, B, T)
     # (a): the staged chain's arrays and state
     nb = dict(rot=9, rz=9, x0=12, ia=3, ig=3, fpr=12, fvr=12, jac=36, foot=12, kpl=3, des=12, ref=9, gc=4, trel=12, fk=12, f_body=12, tau=12)
     dv = {k: eng.dalloc(n * B * 8) for k, n in nb.items()}
@@ -153,21 +209,10 @@ def bench_size(eng, B, repeats, ticks):
         fused()
     eng.sync()
 
-    def timed(fn, k):
-        e0, e1 = eng.event(), eng.event()
-        eng.record(e0)
-        for _ in range(k):
-            fn()
-        eng.record(e1)
-        ms = eng.elapsed_ms(e0, e1) / k
-        for e in (e0, e1):
-            L.a1mpc_event_destroy(eng.h, e)
-        return ms
-
     ta, tb = [], []
     for _ in range(repeats):
-        ta.append(timed(staged, T))
-        tb.append(timed(fused, T))
+        ta.append(timed(eng, staged, T))
+        tb.append(timed(eng, fused, T))
     # (c) per-stage breakdown of (a): one window of T back-to-back ticks, as (a) times them, with an event at every stage boundary and no
     # synchronisation inside; a stage's time is the interval from the previous boundary to its own, so the intervals add up to the window
     ev = [eng.event() for _ in range(len(STAGES) * T + 1)]
@@ -212,14 +257,24 @@ def main():
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--ticks", type=int, default=20)
     ap.add_argument("--json", default=None, help="also write the record here")
+    ap.add_argument("--sched", action="store_true", help="time the scheduled tick against the held-pattern tick")
     a = ap.parse_args()
     if a.ticks < 12:
         ap.error("--ticks must be at least 12 (standstill, walking, standstill in every window)")
     dev = device_line()
     print("device:", dev, flush=True)
     eng = a1mpc.Engine(a1mpc.default_config())
-    rec = dict(device=dev, repeats=a.repeats, ticks=a.ticks, results=[])
+    rec = dict(device=dev, repeats=a.repeats, ticks=a.ticks, results=[], **(dict(mode="sched") if a.sched else {}))
     for B in [int(s) for s in a.sizes.split(",")]:
+        if a.sched:
+            r = bench_sched(eng, B, a.repeats, a.ticks)
+            rec["results"].append(r)
+            f = lambda k: "%.4f ms [%.4f-%.4f]" % (r[k]["ms_median"], r[k]["ms_min"], r[k]["ms_max"])
+            print("B=%6d  held-pattern tick %s | scheduled tick %s" % (B, f("held"), f("sched")), flush=True)
+            for w in ("held", "sched"):
+                print("         (e) kernel time per tick, %s (ms): " % w + ", ".join("%s %.4f" % kv for kv in sorted(r["kernel_ms_per_tick"][w].items())),
+                      flush=True)
+            continue
         r = bench_size(eng, B, a.repeats, a.ticks)
         rec["results"].append(r)
         f = lambda k: "%.4f ms [%.4f-%.4f]" % (r[k]["ms_median"], r[k]["ms_min"], r[k]["ms_max"])
