@@ -22,7 +22,7 @@ EXPORTS = [
     "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
     "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch",
     "a1mpc_imu_bytes", "a1mpc_imu_init_batch", "a1mpc_orientation_batch", "a1mpc_command_bytes", "a1mpc_command_init_batch", "a1mpc_command_batch",
-    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_run", "a1mpc_tick_destroy",
+    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_run", "a1mpc_tick_destroy",
     "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
@@ -187,6 +187,7 @@ def lib():
         l.a1mpc_default_tick_params.argtypes = [C.c_int, C.c_int, C.POINTER(TickParams)]
         l.a1mpc_tick_create.argtypes = [C.c_void_p, C.c_int, C.POINTER(TickParams), C.POINTER(C.c_void_p)]
         l.a1mpc_tick_reset.argtypes = [C.c_void_p]
+        l.a1mpc_tick_reset_robots.argtypes = [C.c_void_p, C.c_void_p]
         l.a1mpc_tick_run.argtypes = [C.c_void_p, C.c_double, C.POINTER(TickInputs), C.POINTER(TickOutputs)]
         l.a1mpc_tick_destroy.argtypes = [C.c_void_p]
         l.a1mpc_gen_states.argtypes = [C.c_int, C.c_uint64, C.c_int] + [C.c_void_p] * 5
@@ -321,6 +322,20 @@ class Tick:
 
     def reset(self):
         _check(lib().a1mpc_tick_reset(self.t))
+
+    def reset_robots(self, mask):
+        """a1mpc_tick_reset_robots on a host mask: numpy bool or uint8 [B]; robot b with mask[b] != 0 starts over as after reset(), the
+        others keep their state.  Copies the mask and synchronises; reset_robots_ptr takes a device mask without either"""
+        m = np.asarray(mask)
+        if m.dtype not in (np.bool_, np.uint8) or m.shape != (self.B,):
+            raise ValueError("mask must be a bool or uint8 array of shape (%d,)" % self.B)
+        m = np.ascontiguousarray(m).view(np.uint8)
+        self.reset_robots_ptr(m.ctypes.data)
+
+    def reset_robots_ptr(self, ptr):
+        """a1mpc_tick_reset_robots on a pointer to B uint8 / bool, e.g. a torch bool tensor's data_ptr(): device memory only enqueues work on
+        the handle's stream, host memory is copied and synchronised"""
+        _check(lib().a1mpc_tick_reset_robots(self.t, ptr))
 
     def close(self):
         """a1mpc_tick_destroy; a tick whose Engine is closed has already been destroyed by Engine.close"""

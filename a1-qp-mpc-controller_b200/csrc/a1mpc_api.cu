@@ -940,6 +940,7 @@ struct a1mpc_tick {
   int B = 0;
   a1mpc_tick_params tp;
   bool first = true;      // the next run initialises the EKF instead of updating it
+  bool pending = false;   // a partial reset has flagged robots in `reset` whose EKF the next run initialises
   void* mem = nullptr;    // one device allocation holding everything below
   // intermediates, dense [rows][B]
   double *rot, *rz, *x0, *ia, *ig, *fpr, *fvr, *jac, *foot, *kpl, *des, *ref, *fk, *f_body;
@@ -949,6 +950,7 @@ struct a1mpc_tick {
   // state
   double *gc, *tau, *imu, *cmd, *swing, *ekf;
   uint32_t* warm;
+  uint8_t* reset;         // [B]: robot reset by a1mpc_tick_reset_robots since the last run (ekf_init_pending)
 };
 
 namespace {
@@ -971,7 +973,9 @@ int tick_reset_impl(a1mpc_tick* t) {
   h->launches += 2;
   CK(cudaGetLastError());
   if (t->warm) CK(cudaMemsetAsync(t->warm, 0, a1mpc_warm_bytes(h, B), h->stream));
+  CK(cudaMemsetAsync(t->reset, 0, lb, h->stream));   // the EKF init of every robot supersedes a pending partial one
   t->first = true;
+  t->pending = false;
   return A1MPC_OK;
 }
 
@@ -1090,6 +1094,7 @@ int a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc
   bytes += 5 * pad(lb * 4);
   if (sched) bytes += pad((size_t)h->cfg.horizon * lb * 4);
   if (warm) bytes += pad(a1mpc_warm_bytes(h, B));
+  bytes += pad(lb);
   a1mpc_tick* t = new a1mpc_tick();
   t->h = h; t->B = B; t->tp = *tp;
   if (cudaMalloc(&t->mem, bytes) != cudaSuccess) {
@@ -1109,6 +1114,7 @@ int a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc
   t->est_status = reinterpret_cast<int32_t*>(take(lb * 4));
   t->sched = sched ? reinterpret_cast<uint32_t*>(take((size_t)h->cfg.horizon * lb * 4)) : nullptr;
   t->warm = warm ? reinterpret_cast<uint32_t*>(take(a1mpc_warm_bytes(h, B))) : nullptr;
+  t->reset = reinterpret_cast<uint8_t*>(take(lb));
   int rc;
   // the scheduled solve's record queues too, so that a run allocates nothing
   if ((rc = ensure_capacity(h, B)) || (sched && (rc = ensure_capacity_ext(h, B))) || (rc = ensure_lists(h, stance_scratch_bytes(B))) ||
@@ -1123,6 +1129,26 @@ int a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc
 int a1mpc_tick_reset(a1mpc_tick* t) {
   if (!t) return fail(A1MPC_EINVAL, "null argument");
   return tick_reset_impl(t);
+}
+
+int a1mpc_tick_reset_robots(a1mpc_tick* t, const uint8_t* mask) {
+  if (!t || !mask) return fail(A1MPC_EINVAL, "null argument");
+  a1mpc_handle* h = t->h;
+  const int B = t->B;
+  CK(cudaSetDevice(h->device));
+  Stage st(h, B);
+  st.in(mask, 1);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  // before the first run after create or reset every robot's EKF is initialised anyway: no flags then
+  const bool flag = !t->first;
+  tick_reset_robots_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, mask, command_init_params(t->tp.command), t->x0, t->gc, t->tau, t->imu, t->cmd,
+                                                                    t->tp.mode == A1MPC_TICK_MPC ? t->ref : nullptr, t->swing, t->warm,
+                                                                    WARM_HDR + 4 * h->cfg.horizon, flag ? t->reset : nullptr);
+  h->launches++;
+  CK(cudaGetLastError());
+  t->pending = t->pending || flag;
+  return st.finish();
 }
 
 int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out) {
@@ -1184,8 +1210,14 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
   } else if ((rc = enqueue_ekf_update(h, B, t->ekf, EkfParams{dt, tp.assume_flat_ground ? 1 : 0}, t->mode, t->ia, t->ig, t->rot, t->fpr, t->fvr, ff,
                                       t->x0 + 3 * lb, t->x0 + 9 * lb, t->est_contacts, t->est_status))) {
     return rc;
+  } else if (t->pending) {
+    // robots reset by a1mpc_tick_reset_robots: the init over the update, as on their first run
+    ekf_init_pending<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->reset, t->ekf, t->fpr, t->rot, t->x0);
+    h->launches++;
+    CK(cudaGetLastError());
   }
   t->first = false;
+  t->pending = false;
   // 7: terrain pitch and the MPC solve, or the stance QP
   if (mpc) {
     terrain_pitch_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->swing, tp.use_terrain_adapt ? 1 : 0, t->x0 + 3 * lb, t->ref, lb, nullptr);

@@ -20,12 +20,7 @@ cudaError_t orientation_launch(int B, const double* quat, const double* gyro, co
 }
 
 cudaError_t command_init_launch(int B, const a1mpc_command_params& cp, double* state, double* ref, size_t ref_ld, cudaStream_t st) {
-  CommandInit P;
-  P.height = cp.body_height; P.hmin = cp.body_height_min; P.hmax = cp.body_height_max;
-  for (int i = 0; i < 3; ++i) P.kp[i] = cp.kp_linear[i];
-  P.lock[0] = cp.kp_linear_lock[0]; P.lock[1] = cp.kp_linear_lock[1];
-  P.variant = cp.variant;
-  command_init_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, P, state, ref, ref_ld);
+  command_init_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, command_init_params(cp), state, ref, ref_ld);
   return cudaGetLastError();
 }
 

@@ -189,9 +189,8 @@ __device__ __forceinline__ void chol_solve8_impl(const double* __restrict__ L, d
 }
 
 // A1BasicEKF::init_state (A1BasicEKF.cpp:56-68): P = 3 I, x = (0,0,0.09, 0,0,0, R fk_i + pos)
-__global__ void ekf_init_kernel(int B, double* __restrict__ state, const double* __restrict__ foot_pos_rel, const double* __restrict__ rot) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+__device__ __forceinline__ void ekf_init_body(int b, int B, double* __restrict__ state, const double* __restrict__ foot_pos_rel,
+                                              const double* __restrict__ rot) {
   const size_t ld = (size_t)B;
   double* x = state + (size_t)b * EKF_STATE_DOUBLES;
   double* P = x + EKF_NX;
@@ -205,6 +204,12 @@ __global__ void ekf_init_kernel(int B, double* __restrict__ state, const double*
     for (int a = 0; a < 3; ++a) p[a] = foot_pos_rel[(size_t)(3 * leg + a) * ld + b];
     for (int a = 0; a < 3; ++a) x[6 + 3 * leg + a] = R[3 * a] * p[0] + R[3 * a + 1] * p[1] + R[3 * a + 2] * p[2] + x[a];
   }
+}
+
+__global__ void ekf_init_kernel(int B, double* __restrict__ state, const double* __restrict__ foot_pos_rel, const double* __restrict__ rot) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  ekf_init_body(b, B, state, foot_pos_rel, rot);
 }
 
 // A1BasicEKF::update_estimation (A1BasicEKF.cpp:70-164).  Inputs batch-major SoA (ld = B).  status[b] = 0, or 3 when S is

@@ -53,10 +53,14 @@ __device__ __forceinline__ double sw_bezier(double t, const double (&P)[5]) {
 }
 
 // zero state = A1CtrlStates::reset() values of the fields above (A1CtrlStates.h:83-100) and fresh filters (A1RobotControl.cpp:52-57)
+__device__ __forceinline__ void swing_init_body(int b, int B, double* __restrict__ state) {
+  for (int f = 0; f < SW_FIELDS; ++f) state[(size_t)f * B + b] = 0.0;
+}
+
 __global__ void swing_init_kernel(int B, double* __restrict__ state) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  for (int f = 0; f < SW_FIELDS; ++f) state[(size_t)f * B + b] = 0.0;
+  swing_init_body(b, B, state);
 }
 
 // one leg of generate_swing_legs_ctrl (A1RobotControl.cpp:204-287) for the robot whose swing state starts at s.  src gives the stage's

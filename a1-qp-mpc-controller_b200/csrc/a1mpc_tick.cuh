@@ -8,12 +8,14 @@
 // also writes the schedule of the scheduled tick.  The stored outputs are the ones later
 // stages read: foot_pos_rel, foot_vel_rel and jac (EKF, torques), foot_pos_abs (the solve's foot), f_kin and contacts (solve, torques), and
 // the gait counters and swing state (next tick).
+// Also the two kernels of a per-robot reset (a1mpc_tick_reset_robots): tick_reset_robots_kernel, and ekf_init_pending in the next run.
 // Bit-identity with the staged kernels: the compiler contracts products into FMAs per kernel, so every stage keeps the loop shape it has
 // in its own kernel.  The foothold targets and the swing legs run in one rolled leg loop, as both do in update_plan_kernel and
 // swing_legs_kernel: unrolled, the foothold's loop-invariant product kf * (v - vd) is no longer hoisted and the other product of dx / dy gets
 // contracted, which moves the targets by an ulp.  The loop index then selects each leg's registers instead of indexing an array, which would
 // go to local memory.
 #pragma once
+#include "a1mpc_command_state.cuh"
 #include "a1mpc_estim.cuh"
 #include "a1mpc_misc.cuh"
 #include "a1mpc_swing.cuh"
@@ -103,6 +105,39 @@ __global__ void tick_front_sched(int B, LegParams LP, GaitDev G, SwingParams SP,
                                  double* __restrict__ fkin, uint32_t* __restrict__ contacts, uint32_t* __restrict__ sched) {
   tick_front_b_body(B, LP, G, SP, joint_pos, joint_vel, rot, rot_z, x0, lin_vel_d, mode, gc, gcs, swing_state, foot_force, fpr, jac, fvr, foot, fkin,
                     contacts, sched);
+}
+
+// a1mpc_tick_reset_robots: robot b with mask[b] != 0 gets the start values a1mpc_tick_reset writes (zero x0, gait counters, tau and warm
+// slot; the bodies of imu_init_kernel, command_init_kernel and swing_init_kernel), and pending[b] = 1 so that the next run initialises its
+// EKF (ekf_init_pending).  imu, ref, warm and pending may be null.  Thread per robot: the warp reads 32 mask bytes at once and every
+// batch-major store of a fully masked warp is coalesced; an unmasked robot costs its mask byte, so k reset robots cost k robots' stores.
+__global__ void tick_reset_robots_kernel(int B, const uint8_t* __restrict__ mask, CommandInit P, double* __restrict__ x0, double* __restrict__ gc,
+                                         double* __restrict__ tau, double* __restrict__ imu, double* __restrict__ cmd, double* __restrict__ ref,
+                                         double* __restrict__ swing, uint32_t* __restrict__ warm, int warm_words, uint8_t* __restrict__ pending) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B || !mask[b]) return;
+  const size_t lb = (size_t)B;
+  for (int r = 0; r < 12; ++r) { x0[r * lb + b] = 0.0; tau[r * lb + b] = 0.0; }
+  for (int r = 0; r < 4; ++r) gc[r * lb + b] = 0.0;
+  if (imu) imu_init_body(b, B, imu);
+  command_init_body(b, B, P, cmd, ref, lb);
+  swing_init_body(b, B, swing);
+  if (warm)
+    for (int w = 0; w < warm_words; ++w) warm[(size_t)b * warm_words + w] = 0u;
+  if (pending) pending[b] = 1;
+}
+
+// stage 6 of the first run after a partial reset, behind the EKF update of every robot: robot b with pending[b] != 0 gets the EKF
+// initialisation of ekf_init_kernel instead of the update, and x0 rows 3-5 and 9-11 back at zero, as on the first run of a fresh tick;
+// pending[b] is cleared.
+__global__ void ekf_init_pending(int B, uint8_t* __restrict__ pending, double* __restrict__ state, const double* __restrict__ foot_pos_rel,
+                                 const double* __restrict__ rot, double* __restrict__ x0) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B || !pending[b]) return;
+  ekf_init_body(b, B, state, foot_pos_rel, rot);
+  const size_t lb = (size_t)B;
+  for (int a = 0; a < 3; ++a) { x0[(3 + a) * lb + b] = 0.0; x0[(9 + a) * lb + b] = 0.0; }
+  pending[b] = 0;
 }
 
 }  // namespace a1mpc

@@ -419,7 +419,9 @@ int  a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, con
  * the previous torques) and every intermediate array, and runs the stages above in the order of one main_update + compute_grf +
  * compute_joint_torques pass:
  *   1 orientation (the IMU filters of the Gazebo and Isaac adapters; none for A1MPC_VARIANT_HARDWARE)   2 leg kinematics   3 command
- *   4 update_plan   5 swing legs   6 EKF: a1mpc_ekf_init_batch on the first run after create or reset, the update after that
+ *   4 update_plan   5 swing legs   6 EKF: a1mpc_ekf_init_batch on the first run after create or reset, the update after that; a robot
+ *     reset by a1mpc_tick_reset_robots since the last run gets the init instead of the update (its x0 rows 3-5 and 9-11 stay zero on
+ *     that run, as on a fresh tick's first run)
  *   7 A1MPC_TICK_MPC: terrain pitch, then the MPC solve, posed one of two ways by gait.horizon:
  *     0 (the default): the contact pattern held over the horizon as compute_grf poses it: the solve of a1mpc_solve_batch_warm with
  *       shift 0 (horizon 10) or the cold a1mpc_solve_batch (horizon 20).  It takes part in the fused collect (a1mpc_peer_gather_*) exactly
@@ -479,6 +481,13 @@ typedef struct a1mpc_tick_outputs {
 int  a1mpc_default_tick_params(int variant, int mode, a1mpc_tick_params* tp);
 int  a1mpc_tick_create(a1mpc_handle* h, int B, const a1mpc_tick_params* tp, a1mpc_tick** out);
 int  a1mpc_tick_reset(a1mpc_tick* t);
+/* Put the robots b with mask[b] != 0 back where a1mpc_tick_create / a1mpc_tick_reset put them; every other robot's state is untouched, so
+ * a simulator can restart one environment's episode while the rest of the batch keeps walking.  mask [B] (uint8: a numpy / torch bool
+ * array passes as is), host or device memory.  Device: enqueued only, no allocation, no synchronisation.  Host: copied, then the same,
+ * and the call synchronises.  The next a1mpc_tick_run initialises the EKF of the reset robots instead of updating it, exactly as the
+ * first run after create does for all robots.  Several calls before one run reset the union of their masks; a1mpc_tick_reset
+ * supersedes a pending partial reset; an all-zero mask changes nothing.  A1MPC_EINVAL: a NULL tick or mask. */
+int  a1mpc_tick_reset_robots(a1mpc_tick* t, const uint8_t* mask);
 int  a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out);
 int  a1mpc_tick_destroy(a1mpc_tick* t);
 
