@@ -20,9 +20,9 @@ EXPORTS = [
     "a1mpc_default_config", "a1mpc_create", "a1mpc_destroy", "a1mpc_last_error", "a1mpc_device_count",
     "a1mpc_solve_batch", "a1mpc_warm_bytes", "a1mpc_warm_reset", "a1mpc_solve_batch_warm", "a1mpc_solve_batch_ext", "a1mpc_solve_batch_ext_warm", "a1mpc_build_qp_batch", "a1mpc_qp_mats_batch", "a1mpc_solve_dense_batch",
     "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
-    "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch",
+    "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_terrain_normals_batch",
     "a1mpc_imu_bytes", "a1mpc_imu_init_batch", "a1mpc_orientation_batch", "a1mpc_command_bytes", "a1mpc_command_init_batch", "a1mpc_command_batch",
-    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_run", "a1mpc_tick_destroy",
+    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_set_terrain", "a1mpc_tick_run", "a1mpc_tick_destroy",
     "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
@@ -80,6 +80,7 @@ def default_command_params(variant=VARIANT_GAZEBO):
 
 
 TICK_QP, TICK_MPC = 0, 1
+TERRAIN_FLAT, TERRAIN_ESTIMATED, TERRAIN_GIVEN = 0, 1, 2   # a1mpc_tick_set_terrain
 
 
 class TickParams(C.Structure):
@@ -176,6 +177,8 @@ def lib():
         l.a1mpc_swing_init_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         l.a1mpc_swing_legs_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_double] + [C.c_void_p] * 10
         l.a1mpc_terrain_pitch_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        l.a1mpc_terrain_normals_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                  C.c_void_p]
         for name in ("a1mpc_imu_bytes", "a1mpc_command_bytes"):
             getattr(l, name).restype = C.c_size_t
             getattr(l, name).argtypes = [C.c_int]
@@ -188,6 +191,7 @@ def lib():
         l.a1mpc_tick_create.argtypes = [C.c_void_p, C.c_int, C.POINTER(TickParams), C.POINTER(C.c_void_p)]
         l.a1mpc_tick_reset.argtypes = [C.c_void_p]
         l.a1mpc_tick_reset_robots.argtypes = [C.c_void_p, C.c_void_p]
+        l.a1mpc_tick_set_terrain.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         l.a1mpc_tick_run.argtypes = [C.c_void_p, C.c_double, C.POINTER(TickInputs), C.POINTER(TickOutputs)]
         l.a1mpc_tick_destroy.argtypes = [C.c_void_p]
         l.a1mpc_gen_states.argtypes = [C.c_int, C.c_uint64, C.c_int] + [C.c_void_p] * 5
@@ -284,7 +288,9 @@ class Tick:
 
     In MPC mode params.gait.horizon picks how the solve is posed: 0 (the default) holds the current contact pattern over the horizon as
     the reference does; the engine's horizon runs the scheduled tick, whose solve sees the gait's planned contacts over the horizon (step 0
-    the swing stage's contacts) and does not take part in the fused collect.  Any other value is rejected; QP mode ignores it."""
+    the swing stage's contacts) and does not take part in the fused collect.  Any other value is rejected; QP mode ignores it.
+    set_terrain picks where the MPC solve's friction pyramids stand: world z (the default), the estimated walking surface or the caller's
+    normals."""
 
     _SHAPES = dict(quat=(4,), gyro=(3,), acc=(3,), joint_pos=(12,), joint_vel=(12,), foot_force=(4,), cmd=(7,), gait_counter_speed=(4,))
 
@@ -336,6 +342,12 @@ class Tick:
         """a1mpc_tick_reset_robots on a pointer to B uint8 / bool, e.g. a torch bool tensor's data_ptr(): device memory only enqueues work on
         the handle's stream, host memory is copied and synchronised"""
         _check(lib().a1mpc_tick_reset_robots(self.t, ptr))
+
+    def set_terrain(self, source, normals_ptr=0):
+        """a1mpc_tick_set_terrain: TERRAIN_FLAT (world-z pyramids, the default), TERRAIN_ESTIMATED (the terrain stage's fitted surface
+        normal) or TERRAIN_GIVEN with normals_ptr a device pointer to [12][B] float64 per-foot normals, e.g. a torch tensor's data_ptr(),
+        read by every later run.  MPC mode only for the non-flat sources"""
+        _check(lib().a1mpc_tick_set_terrain(self.t, int(source), normals_ptr or None))
 
     def close(self):
         """a1mpc_tick_destroy; a tick whose Engine is closed has already been destroyed by Engine.close"""
@@ -565,6 +577,19 @@ class Engine:
         _check(lib().a1mpc_terrain_pitch_batch(self.h, B, swing, int(use_terrain_adapt), _p(pos), _p(ref), ref.shape[1] if ref is not None else B,
                                                _p(pitch)))
         return pitch
+
+    def terrain_normals(self, swing, use_terrain_adapt, root_pos, ref=None):
+        """a1mpc_terrain_normals_batch, host arrays: terrain_pitch plus the walking surface's unit normal -> (terrain_pitch [B],
+        normals [12,B], the same for all four feet)"""
+        pos = np.ascontiguousarray(root_pos, dtype=np.float64)
+        B = pos.shape[1]
+        if ref is not None and not (ref.dtype == np.float64 and ref.flags["C_CONTIGUOUS"]):
+            raise A1MpcError("ref must be a C-contiguous float64 array (written in place)")
+        pitch = np.zeros(B)
+        normals = np.zeros((12, B))
+        _check(lib().a1mpc_terrain_normals_batch(self.h, B, swing, int(use_terrain_adapt), _p(pos), _p(ref), ref.shape[1] if ref is not None else B,
+                                                 _p(pitch), _p(normals)))
+        return pitch, normals
 
     def imu_alloc(self, B):
         """device-resident IMU filter state of B robots (a1mpc_imu_bytes), initialised by a1mpc_imu_init_batch; bound to this B"""

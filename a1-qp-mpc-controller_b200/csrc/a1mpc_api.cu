@@ -856,6 +856,29 @@ int a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use
   return st.finish();
 }
 
+int a1mpc_terrain_normals_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref, size_t ref_ld,
+                                double* terrain_pitch, double* normals) {
+  if (!h || !swing_state || !root_pos || !normals || (use_terrain_adapt && !ref)) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (ref && ref_ld < (size_t)B) return fail(A1MPC_EINVAL, "ref_ld must be >= B");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
+  double* row = use_terrain_adapt ? ref + ref_ld : nullptr;   // as in a1mpc_terrain_pitch_batch
+  Stage st(h, B);
+  st.in(root_pos, 3);
+  st.out(row, 1); st.out(terrain_pitch, 1); st.out(normals, 12);
+  if (!use_terrain_adapt) st.unused(ref);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  double* kref = st.host() ? row : ref;
+  const size_t kld = st.host() ? 0 : ref_ld;
+  terrain_normals_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, static_cast<double*>(swing_state), use_terrain_adapt ? 1 : 0, root_pos, kref,
+                                                                 kld, terrain_pitch, normals, nullptr, nullptr, 0);
+  h->launches++;
+  CK(cudaGetLastError());
+  return st.finish();
+}
+
 // ---- orientation and command stages (the adapters' IMU / pose callbacks and main_update's front half) ------------------------
 size_t a1mpc_imu_bytes(int B) { return B > 0 ? (size_t)B * imu_state_doubles() * sizeof(double) : 0; }
 
@@ -951,6 +974,12 @@ struct a1mpc_tick {
   double *gc, *tau, *imu, *cmd, *swing, *ekf;
   uint32_t* warm;
   uint8_t* reset;         // [B]: robot reset by a1mpc_tick_reset_robots since the last run (ekf_init_pending)
+  // the solve's friction pyramids (a1mpc_tick_set_terrain)
+  int terrain = A1MPC_TERRAIN_FLAT;
+  const double* given = nullptr;   // A1MPC_TERRAIN_GIVEN: the caller's normals [12][B]
+  void* tmem = nullptr;            // allocated by the first set_terrain to a non-flat source: normals, then held
+  double* normals = nullptr;       // [12][B] terrain_normals_kernel's estimate
+  uint32_t* held = nullptr;        // [N][B] the held pattern as a schedule (gait.horizon = 0), else NULL
 };
 
 namespace {
@@ -1151,6 +1180,41 @@ int a1mpc_tick_reset_robots(a1mpc_tick* t, const uint8_t* mask) {
   return st.finish();
 }
 
+int a1mpc_tick_set_terrain(a1mpc_tick* t, int source, const double* normals) {
+  if (!t) return fail(A1MPC_EINVAL, "null argument");
+  if (source != A1MPC_TERRAIN_FLAT && source != A1MPC_TERRAIN_ESTIMATED && source != A1MPC_TERRAIN_GIVEN) return fail(A1MPC_EINVAL, "unknown terrain source");
+  if (source == A1MPC_TERRAIN_FLAT) {
+    t->terrain = source;
+    t->given = nullptr;
+    return A1MPC_OK;
+  }
+  a1mpc_handle* h = t->h;
+  if (t->tp.mode != A1MPC_TICK_MPC) return fail(A1MPC_EINVAL, "terrain normals need MPC mode (the stance QP keeps its world-z pyramid)");
+  for (int i = 0; i < 4; ++i)
+    if (h->cfg.r[3 * i] != h->cfg.r[3 * i + 1] || h->cfg.r[3 * i] != h->cfg.r[3 * i + 2])
+      return fail(A1MPC_EINVAL, "terrain normals need isotropic r weights per foot (r[3i] == r[3i+1] == r[3i+2])");
+  if (source == A1MPC_TERRAIN_GIVEN && !normals) return fail(A1MPC_EINVAL, "A1MPC_TERRAIN_GIVEN needs a normals array");
+  CK(cudaSetDevice(h->device));
+  if (source == A1MPC_TERRAIN_GIVEN && !is_device_ptr(normals)) return fail(A1MPC_EINVAL, "the given normals must be device memory");
+  const size_t lb = (size_t)t->B;
+  if (!t->tmem) {
+    auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t nb = pad(12 * lb * sizeof(double)), sb = t->sched ? 0 : (size_t)h->cfg.horizon * lb * 4;
+    if (cudaMalloc(&t->tmem, nb + sb) != cudaSuccess) {
+      cudaGetLastError();
+      t->tmem = nullptr;
+      return fail(A1MPC_ENOMEM, "cudaMalloc failed");
+    }
+    t->normals = static_cast<double*>(t->tmem);
+    t->held = sb ? reinterpret_cast<uint32_t*>(static_cast<char*>(t->tmem) + nb) : nullptr;
+  }
+  int rc;
+  if ((rc = ensure_capacity_ext(h, lb))) return rc;   // so that a run allocates nothing
+  t->terrain = source;
+  t->given = source == A1MPC_TERRAIN_GIVEN ? normals : nullptr;
+  return A1MPC_OK;
+}
+
 int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out) {
   if (!t || !in || !out || !out->tau) return fail(A1MPC_EINVAL, "null argument");
   if (!in->quat || !in->gyro || !in->acc || !in->joint_pos || !in->joint_vel || !in->foot_force || !in->cmd || !in->gait_counter_speed)
@@ -1173,7 +1237,7 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
   if ((rc = st.begin())) return rc;
   if ((rc = ensure_capacity(h, B))) return rc;   // create sized the scratch and it only grows: no allocation here
   if (!mpc && (rc = ensure_lists(h, stance_scratch_bytes(B)))) return rc;
-  if (t->sched && (rc = ensure_capacity_ext(h, B))) return rc;
+  if ((t->sched || t->tmem) && (rc = ensure_capacity_ext(h, B))) return rc;
   const a1mpc_tick_params& tp = t->tp;
   // 1-3: orientation and command
   CK(tick_front_a_launch(B, dt, quat, gyro, acc, t->imu, t->rot, t->rz, t->x0, t->ia, t->ig, t->cmd, cmd, t->mode, t->kpl, mpc ? t->ref : nullptr,
@@ -1219,7 +1283,19 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
   t->first = false;
   t->pending = false;
   // 7: terrain pitch and the MPC solve, or the stance QP
-  if (mpc) {
+  if (mpc && t->terrain != A1MPC_TERRAIN_FLAT) {
+    // the same stage plus the estimated normals (and the held pattern as a schedule), then the solve of a1mpc_solve_batch_ext_warm
+    // with normals: shift 1 on the scheduled tick's schedule, shift 0 on the held one (a1mpc_solve_batch_ext at horizon 20)
+    terrain_normals_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->swing, tp.use_terrain_adapt ? 1 : 0, t->x0 + 3 * lb, t->ref, lb, nullptr,
+                                                                   t->normals, t->contact, t->held, h->cfg.horizon);
+    h->launches++;
+    CK(cudaGetLastError());
+    const DevInputs di{t->x0, t->rot, t->foot, t->ref, t->contact, lb, 0};
+    const DevOutputs dout{t->f_body, t->status, nullptr, nullptr, lb, 0};
+    const double* nrm = t->terrain == A1MPC_TERRAIN_GIVEN ? t->given : t->normals;
+    if ((rc = t->sched ? enqueue_solve_ext(h, B, di, t->sched, nrm, dout, t->warm, 1) : enqueue_solve_ext(h, B, di, t->held, nrm, dout, t->warm, 0)))
+      return rc;
+  } else if (mpc) {
     terrain_pitch_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->swing, tp.use_terrain_adapt ? 1 : 0, t->x0 + 3 * lb, t->ref, lb, nullptr);
     h->launches++;
     CK(cudaGetLastError());
@@ -1260,6 +1336,7 @@ int a1mpc_tick_destroy(a1mpc_tick* t) {
   cudaSetDevice(t->h->device);
   cudaStreamSynchronize(t->h->stream);
   if (t->mem) cudaFree(t->mem);
+  if (t->tmem) cudaFree(t->tmem);
   delete t;
   return A1MPC_OK;
 }

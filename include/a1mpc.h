@@ -334,6 +334,12 @@ int  a1mpc_update_plan_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp
  *                              0.05 m above the rear ones.  root_pos [3][B]; ref [9][B] with leading dimension ref_ld >= B, an
  *                              a1mpc_inputs.ref array: only row 1 (root_euler_d[1]) is written, and only when use_terrain_adapt (ref may
  *                              be NULL otherwise); terrain_pitch [B] out (terrain_pitch_angle, may be NULL).
+ *   a1mpc_terrain_normals_batch  a1mpc_terrain_pitch_batch (the same filter update, ref row 1 and terrain_pitch) that also writes
+ *                              normals [12][B] (mandatory): the walking surface's unit normal in the world frame, the same for all four
+ *                              feet, as the per-foot normals of a1mpc_solve_batch_ext take it.  It is the fitted plane's own normal
+ *                              (-a1, -a2, 1) / |.| (z = a0 + a1 x + a2 y in the frame of foot_pos_recent_contact, which has world
+ *                              axes), its tilt clipped to 0.5 rad about the same horizontal axis, and e_z while root_pos z <= 0.1;
+ *                              so n_z >= cos 0.5 > 0.  It advances the same filter: a chain calls one of the two, never both.
  */
 size_t a1mpc_swing_bytes(int B);
 int  a1mpc_swing_init_batch(a1mpc_handle* h, int B, void* swing_state);
@@ -343,6 +349,8 @@ int  a1mpc_swing_legs_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp,
                             double* foot_pos_recent_contact);
 int  a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref, size_t ref_ld,
                                double* terrain_pitch);
+int  a1mpc_terrain_normals_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref,
+                                 size_t ref_ld, double* terrain_pitch, double* normals);
 
 /* ---- the first two stages of a control tick: the adapters' orientation and command stages ---------------------------------
  * Together with the stages above they let a whole tick run from raw sensor arrays on device pointers.  One thread per robot;
@@ -431,6 +439,7 @@ int  a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, con
  *       schedule [N][B] of a1mpc_update_plan_batch, whose step 0 is replaced by the swing stage's contacts (plan OR early contact: the
  *       feet the torque stage treats as stance), world-z friction pyramids (no normals).  Like a1mpc_solve_batch_ext it does not take
  *       part in the fused collect.  The schedule stays inside the tick.
+ *     Either way the friction pyramids stand on world z unless a1mpc_tick_set_terrain chose another source (below).
  *     A1MPC_TICK_QP: a1mpc_stance_qp_batch.
  *   8 joint torques.
  * The arrays connect as in a hand-built chain of those entry points: x0 rows 3-5 / 9-11 are the EKF's estimate (zero until its first
@@ -488,6 +497,26 @@ int  a1mpc_tick_reset(a1mpc_tick* t);
  * first run after create does for all robots.  Several calls before one run reset the union of their masks; a1mpc_tick_reset
  * supersedes a pending partial reset; an all-zero mask changes nothing.  A1MPC_EINVAL: a NULL tick or mask. */
 int  a1mpc_tick_reset_robots(a1mpc_tick* t, const uint8_t* mask);
+/* Where an MPC-mode tick's friction pyramids stand (stage 7).  The ground can only push inside a cone about its own normal, so on a slope
+ * the world-z pyramid is the wrong constraint.
+ *   A1MPC_TERRAIN_FLAT       world z, the default: the tick as if this call had never been made (normals ignored).
+ *   A1MPC_TERRAIN_ESTIMATED  the normal of the walking surface the terrain stage fits every tick (a1mpc_terrain_normals_batch), the same
+ *                            for all four feet.
+ *   A1MPC_TERRAIN_GIVEN      normals [12][B]: a caller-owned DEVICE array (per foot, world frame, n_z > 0, e.g. a height-field lookup)
+ *                            that every later run reads at stage 7; the caller orders its writes before the run, as with any device
+ *                            input.  The terrain stage still runs and writes ref row 1 as before.
+ * With ESTIMATED or GIVEN, stage 7 is a1mpc_terrain_normals_batch and then the solve of a1mpc_solve_batch_ext_warm with those normals:
+ * on the scheduled tick's schedule with shift 1; with the held pattern on a schedule of the swing stage's contacts in all N rows with
+ * shift 0 (the cold a1mpc_solve_batch_ext at horizon 20).  Like every _ext solve it does not take part in the fused collect.  Switching
+ * source between runs needs no clean-up: the warm slots of the held-pattern solve and of the _ext solve read each other as "no guess".
+ * The first call to a non-flat source allocates the tick's normals and held schedule and sizes the handle's scratch (it may
+ * synchronise); after it a run on device arrays still allocates nothing and does not synchronise.  a1mpc_tick_reset and
+ * a1mpc_tick_reset_robots keep the source.  A1MPC_EINVAL: a NULL tick, an unknown source, a non-flat source in QP mode (the stance QP
+ * keeps its world-z pyramid) or on a handle with non-isotropic r, GIVEN with a NULL or host pointer. */
+#define A1MPC_TERRAIN_FLAT      0
+#define A1MPC_TERRAIN_ESTIMATED 1
+#define A1MPC_TERRAIN_GIVEN     2
+int  a1mpc_tick_set_terrain(a1mpc_tick* t, int source, const double* normals);
 int  a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out);
 int  a1mpc_tick_destroy(a1mpc_tick* t);
 
