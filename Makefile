@@ -34,6 +34,7 @@ oracle:
 	$(MAKE) -C oracle -s
 	$(MAKE) -C oracle -s -f swing.mk all ref
 	$(MAKE) -C oracle -s -f command.mk all ref
+	$(MAKE) -C oracle -s -f ekf_batch.mk all
 
 host: $(LIB)
 	@if [ -f $(PKG)/host/Makefile ]; then $(MAKE) -C $(PKG)/host -s; fi

@@ -213,7 +213,7 @@ __global__ void ekf_init_kernel(int B, double* __restrict__ state, const double*
 }
 
 // A1BasicEKF::update_estimation (A1BasicEKF.cpp:70-164).  Inputs batch-major SoA (ld = B).  status[b] = 0, or 3 when S is
-// not positive definite / not finite (the state of that robot is then left untouched).
+// not positive definite / not finite or error_y is not finite (the state of that robot is then left untouched).
 __global__ void __launch_bounds__(32 * EKF_WPC) ekf_update_kernel(int B, EkfParams P, double* __restrict__ state,
                                                                  const uint32_t* __restrict__ movement_mode, const double* __restrict__ imu_acc,
                                                                  const double* __restrict__ imu_ang_vel, const double* __restrict__ rot,
@@ -241,8 +241,10 @@ __global__ void __launch_bounds__(32 * EKF_WPC) ekf_update_kernel(int B, EkfPara
     if (lane < 4) {
       const double ff = foot_force[(size_t)lane * ld + b];
       in[39 + lane] = ff;
-      // contact estimation (:78-86): stand -> 1, walk -> clamp(force / 100, 0, 1)
-      in[43 + lane] = (movement_mode[b] == 0u) ? 1.0 : fmin(fmax(ff / (100.0 - 0.0), 0.0), 1.0);
+      // contact estimation (:78-86): stand -> 1, walk -> clamp(force / 100, 0, 1) with the comparisons of std::max / std::min,
+      // so a NaN force stays NaN (fmax / fmin would drop it) and ends the robot NUMERICAL through S
+      const double r = ff / (100.0 - 0.0);
+      in[43 + lane] = (movement_mode[b] == 0u) ? 1.0 : (r < 0.0 ? 0.0 : (1.0 < r ? 1.0 : r));
     }
     __syncwarp();
     const double* R = in; const double* fk = in + 15; const double* fv = in + 27; const double* ec = in + 43;

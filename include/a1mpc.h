@@ -278,7 +278,12 @@ int  a1mpc_leg_kinematics_batch(a1mpc_handle* h, int B, const double* joint_pos,
  *   batch-major SoA inputs (ld = B), host or device: movement_mode [B], imu_acc [3][B], imu_ang_vel [3][B], rot [9][B],
  *   foot_pos_rel [12][B], foot_vel_rel [12][B], foot_force [4][B]
  *   out (any may be NULL): root_pos [3][B] (= estimated_root_pos), root_lin_vel [3][B], estimated_contacts [B] (bit i = leg i),
- *   status [B]: 0, or A1MPC_STATUS_NUMERICAL when S is not positive definite / not finite (that robot's state is untouched). */
+ *   status [B]: 0, or A1MPC_STATUS_NUMERICAL when S is not positive definite / not finite (that robot's state is untouched).
+ *   Non-finite input: a NaN or Inf in imu_acc, imu_ang_vel, rot, foot_pos_rel or foot_vel_rel, or a NaN foot_force in walking
+ *   mode (the contact estimate min(max(force / 100, 0), 1) keeps the NaN, as the reference's std::min / std::max do), makes the
+ *   robot NUMERICAL: its state is untouched, root_pos / root_lin_vel are that state's, and a NaN force's contact bit is 1 (the
+ *   reference's ec < 0.5 test is false for NaN).  +-Inf force in walking mode clamps to contact 1 / 0, and standstill ignores the
+ *   force: neither is NUMERICAL. */
 size_t a1mpc_ekf_bytes(int B);
 int  a1mpc_ekf_init_batch(a1mpc_handle* h, int B, void* ekf_state, const double* foot_pos_rel, const double* rot);
 int  a1mpc_ekf_update_batch(a1mpc_handle* h, int B, void* ekf_state, double dt, int assume_flat_ground, const uint32_t* movement_mode,
