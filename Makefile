@@ -35,6 +35,7 @@ oracle:
 	$(MAKE) -C oracle -s -f swing.mk all ref
 	$(MAKE) -C oracle -s -f command.mk all ref
 	$(MAKE) -C oracle -s -f ekf_batch.mk all
+	$(MAKE) -C oracle -s -f stance_terrain.mk all
 
 host: $(LIB)
 	@if [ -f $(PKG)/host/Makefile ]; then $(MAKE) -C $(PKG)/host -s; fi

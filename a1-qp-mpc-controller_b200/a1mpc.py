@@ -19,10 +19,10 @@ STATUS_OPTIMAL, STATUS_IPM_ONLY, STATUS_MAXITER, STATUS_NUMERICAL, STATUS_NO_CON
 EXPORTS = [
     "a1mpc_default_config", "a1mpc_create", "a1mpc_destroy", "a1mpc_last_error", "a1mpc_device_count",
     "a1mpc_solve_batch", "a1mpc_warm_bytes", "a1mpc_warm_reset", "a1mpc_solve_batch_warm", "a1mpc_solve_batch_ext", "a1mpc_solve_batch_ext_warm", "a1mpc_build_qp_batch", "a1mpc_qp_mats_batch", "a1mpc_solve_dense_batch",
-    "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
-    "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_terrain_normals_batch",
+    "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_stance_qp_batch_ext", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
+    "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_terrain_normals_batch", "a1mpc_surface_normals_batch",
     "a1mpc_imu_bytes", "a1mpc_imu_init_batch", "a1mpc_orientation_batch", "a1mpc_command_bytes", "a1mpc_command_init_batch", "a1mpc_command_batch",
-    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_set_terrain", "a1mpc_tick_run", "a1mpc_tick_destroy",
+    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_set_terrain", "a1mpc_tick_set_stance_terrain", "a1mpc_tick_run", "a1mpc_tick_destroy",
     "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
@@ -170,6 +170,7 @@ def lib():
         l.a1mpc_solve_dense_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
         l.a1mpc_grf_qp_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
         l.a1mpc_stance_qp_batch.argtypes = [C.c_void_p, C.c_int, C.c_size_t] + [C.c_void_p] * 13
+        l.a1mpc_stance_qp_batch_ext.argtypes = [C.c_void_p, C.c_int, C.c_size_t] + [C.c_void_p] * 14
         l.a1mpc_joint_torques_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
         l.a1mpc_update_plan_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams)] + [C.c_void_p] * 13
         l.a1mpc_swing_bytes.restype = C.c_size_t
@@ -179,6 +180,7 @@ def lib():
         l.a1mpc_terrain_pitch_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         l.a1mpc_terrain_normals_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
                                                   C.c_void_p]
+        l.a1mpc_surface_normals_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         for name in ("a1mpc_imu_bytes", "a1mpc_command_bytes"):
             getattr(l, name).restype = C.c_size_t
             getattr(l, name).argtypes = [C.c_int]
@@ -192,6 +194,7 @@ def lib():
         l.a1mpc_tick_reset.argtypes = [C.c_void_p]
         l.a1mpc_tick_reset_robots.argtypes = [C.c_void_p, C.c_void_p]
         l.a1mpc_tick_set_terrain.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        l.a1mpc_tick_set_stance_terrain.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         l.a1mpc_tick_run.argtypes = [C.c_void_p, C.c_double, C.POINTER(TickInputs), C.POINTER(TickOutputs)]
         l.a1mpc_tick_destroy.argtypes = [C.c_void_p]
         l.a1mpc_gen_states.argtypes = [C.c_int, C.c_uint64, C.c_int] + [C.c_void_p] * 5
@@ -290,7 +293,7 @@ class Tick:
     the reference does; the engine's horizon runs the scheduled tick, whose solve sees the gait's planned contacts over the horizon (step 0
     the swing stage's contacts) and does not take part in the fused collect.  Any other value is rejected; QP mode ignores it.
     set_terrain picks where the MPC solve's friction pyramids stand: world z (the default), the estimated walking surface or the caller's
-    normals."""
+    normals; set_stance_terrain does the same for the QP-mode stance QP."""
 
     _SHAPES = dict(quat=(4,), gyro=(3,), acc=(3,), joint_pos=(12,), joint_vel=(12,), foot_force=(4,), cmd=(7,), gait_counter_speed=(4,))
 
@@ -348,6 +351,12 @@ class Tick:
         normal) or TERRAIN_GIVEN with normals_ptr a device pointer to [12][B] float64 per-foot normals, e.g. a torch tensor's data_ptr(),
         read by every later run.  MPC mode only for the non-flat sources"""
         _check(lib().a1mpc_tick_set_terrain(self.t, int(source), normals_ptr or None))
+
+    def set_stance_terrain(self, source, normals_ptr=0):
+        """a1mpc_tick_set_stance_terrain, the QP-mode counterpart of set_terrain: TERRAIN_FLAT (world-z pyramids, the default),
+        TERRAIN_ESTIMATED (the walking surface fitted through the recent-contact points) or TERRAIN_GIVEN with normals_ptr a device pointer to
+        [12][B] float64 per-foot normals, read by every later run.  QP mode only"""
+        _check(lib().a1mpc_tick_set_stance_terrain(self.t, int(source), normals_ptr or None))
 
     def close(self):
         """a1mpc_tick_destroy; a tick whose Engine is closed has already been destroyed by Engine.close"""
@@ -499,6 +508,21 @@ class Engine:
                                            _p(acc)))
         return (f, status, acc) if want_acc else (f, status)
 
+    def stance_qp_ext(self, x0, rot, rot_z, foot, contact, des, kp_linear, kd_linear, kp_angular, kd_angular, normals, want_acc=False):
+        """a1mpc_stance_qp_batch_ext: stance_qp with each stance foot's friction pyramid on its terrain normal, normals [12,B] (per foot, world
+        frame, normalised by the engine) -> f_body [12,B], status [B] (, root_acc [6,B] when want_acc)"""
+        a = [np.ascontiguousarray(v, dtype=np.float64) for v in (x0, rot, rot_z, foot)]
+        contact = np.ascontiguousarray(contact, dtype=np.uint32)
+        d, kpl = np.ascontiguousarray(des, dtype=np.float64), np.ascontiguousarray(kp_linear, dtype=np.float64)
+        g = [np.ascontiguousarray(v, dtype=np.float64) for v in (kd_linear, kp_angular, kd_angular)]
+        nrm = np.ascontiguousarray(normals, dtype=np.float64)
+        B = contact.shape[0]
+        f = np.zeros((12, B)); status = np.zeros(B, dtype=np.int32)
+        acc = np.zeros((6, B)) if want_acc else None
+        _check(lib().a1mpc_stance_qp_batch_ext(self.h, B, B, *[_p(v) for v in a], _p(contact), _p(d), _p(kpl), *[_p(v) for v in g], _p(nrm), _p(f),
+                                               _p(status), _p(acc)))
+        return (f, status, acc) if want_acc else (f, status)
+
     def joint_torques(self, f_grf, f_kin, jac, contact, km_foot, torques_gravity, tau_prev=None):
         """batch-major SoA [12,B], [12,B], [36,B], [B] -> tau [12,B]"""
         a = [np.ascontiguousarray(v, dtype=np.float64) for v in (f_grf, f_kin, jac, km_foot, torques_gravity)]
@@ -590,6 +614,15 @@ class Engine:
         _check(lib().a1mpc_terrain_normals_batch(self.h, B, swing, int(use_terrain_adapt), _p(pos), _p(ref), ref.shape[1] if ref is not None else B,
                                                  _p(pitch), _p(normals)))
         return pitch, normals
+
+    def surface_normals(self, swing, root_pos):
+        """a1mpc_surface_normals_batch, host arrays: the walking surface's unit normal of terrain_normals without the terrain stage (the
+        swing state is only read) -> normals [12,B], the same for all four feet"""
+        pos = np.ascontiguousarray(root_pos, dtype=np.float64)
+        B = pos.shape[1]
+        normals = np.zeros((12, B))
+        _check(lib().a1mpc_surface_normals_batch(self.h, B, swing, _p(pos), _p(normals)))
+        return normals
 
     def imu_alloc(self, B):
         """device-resident IMU filter state of B robots (a1mpc_imu_bytes), initialised by a1mpc_imu_init_batch; bound to this B"""

@@ -647,9 +647,12 @@ int a1mpc_grf_qp_batch(a1mpc_handle* h, int B, const double* root_acc, const dou
   return st.finish();
 }
 
-int a1mpc_stance_qp_batch(a1mpc_handle* h, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
+}  // extern "C"
+
+// a1mpc_stance_qp_batch, and with normals (not NULL) a1mpc_stance_qp_batch_ext
+static int stance_qp_impl(a1mpc_handle* h, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
                           const uint32_t* contact, const double* des, const double* kp_linear, const double* kd_linear, const double* kp_angular,
-                          const double* kd_angular, double* f_body, int32_t* status, double* root_acc) {
+                          const double* kd_angular, const double* normals, double* f_body, int32_t* status, double* root_acc) {
   if (!h || !x0 || !rot || !rot_z || !foot || !contact || !des || !kp_linear || !kd_linear || !kp_angular || !kd_angular || !f_body || !status)
     return fail(A1MPC_EINVAL, "null argument");
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
@@ -657,7 +660,7 @@ int a1mpc_stance_qp_batch(a1mpc_handle* h, int B, size_t ld, const double* x0, c
   CK(cudaSetDevice(h->device));
   Stage st(h, B);
   st.in(x0, 12, 8, ld); st.in(rot, 9, 8, ld); st.in(rot_z, 9, 8, ld); st.in(foot, 12, 8, ld); st.in(contact, 1);
-  st.in(des, 12, 8, ld); st.in(kp_linear, 3, 8, ld);
+  st.in(des, 12, 8, ld); st.in(kp_linear, 3, 8, ld); st.in(normals, 12, 8, ld);
   st.out(f_body, 12, 8, ld); st.out(status, 1); st.out(root_acc, 6, 8, ld);
   st.host_param(kd_linear, "kd_linear"); st.host_param(kp_angular, "kp_angular"); st.host_param(kd_angular, "kd_angular");
   int rc;
@@ -668,12 +671,29 @@ int a1mpc_stance_qp_batch(a1mpc_handle* h, int B, size_t ld, const double* x0, c
   for (int i = 0; i < 3; ++i) { gains[i] = kd_linear[i]; gains[3 + i] = kp_angular[i]; gains[6 + i] = kd_angular[i]; }
   {
     int nl = 0;
-    cudaError_t e = stance_qp_launch(h->sm_count, B, kld, x0, rot, rot_z, foot, contact, des, kp_linear, gains, h->cfg.mass, f_body, status,
-                                     root_acc, h->d_lists, h->stream, &nl);
+    cudaError_t e = stance_qp_launch(h->sm_count, B, kld, x0, rot, rot_z, foot, contact, des, kp_linear, gains, h->cfg.mass, normals, f_body,
+                                     status, root_acc, h->d_lists, h->stream, &nl);
     if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("stance_qp kernels: ") + cudaGetErrorString(e));
     h->launches += nl;
   }
   return st.finish();
+}
+
+extern "C" {
+
+int a1mpc_stance_qp_batch(a1mpc_handle* h, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
+                          const uint32_t* contact, const double* des, const double* kp_linear, const double* kd_linear, const double* kp_angular,
+                          const double* kd_angular, double* f_body, int32_t* status, double* root_acc) {
+  return stance_qp_impl(h, B, ld, x0, rot, rot_z, foot, contact, des, kp_linear, kd_linear, kp_angular, kd_angular, nullptr, f_body, status,
+                        root_acc);
+}
+
+int a1mpc_stance_qp_batch_ext(a1mpc_handle* h, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
+                              const uint32_t* contact, const double* des, const double* kp_linear, const double* kd_linear,
+                              const double* kp_angular, const double* kd_angular, const double* normals, double* f_body, int32_t* status,
+                              double* root_acc) {
+  return stance_qp_impl(h, B, ld, x0, rot, rot_z, foot, contact, des, kp_linear, kd_linear, kp_angular, kd_angular, normals, f_body, status,
+                        root_acc);
 }
 
 int a1mpc_joint_torques_batch(a1mpc_handle* h, int B, const double* f_grf, const double* f_kin, const double* jac, const uint32_t* contact,
@@ -879,6 +899,22 @@ int a1mpc_terrain_normals_batch(a1mpc_handle* h, int B, void* swing_state, int u
   return st.finish();
 }
 
+int a1mpc_surface_normals_batch(a1mpc_handle* h, int B, const void* swing_state, const double* root_pos, double* normals) {
+  if (!h || !swing_state || !root_pos || !normals) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
+  Stage st(h, B);
+  st.in(root_pos, 3);
+  st.out(normals, 12);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  surface_normals_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, static_cast<const double*>(swing_state), root_pos, normals);
+  h->launches++;
+  CK(cudaGetLastError());
+  return st.finish();
+}
+
 // ---- orientation and command stages (the adapters' IMU / pose callbacks and main_update's front half) ------------------------
 size_t a1mpc_imu_bytes(int B) { return B > 0 ? (size_t)B * imu_state_doubles() * sizeof(double) : 0; }
 
@@ -974,11 +1010,11 @@ struct a1mpc_tick {
   double *gc, *tau, *imu, *cmd, *swing, *ekf;
   uint32_t* warm;
   uint8_t* reset;         // [B]: robot reset by a1mpc_tick_reset_robots since the last run (ekf_init_pending)
-  // the solve's friction pyramids (a1mpc_tick_set_terrain)
+  // the friction pyramids of the solve (a1mpc_tick_set_terrain) or of the stance QP (a1mpc_tick_set_stance_terrain)
   int terrain = A1MPC_TERRAIN_FLAT;
   const double* given = nullptr;   // A1MPC_TERRAIN_GIVEN: the caller's normals [12][B]
-  void* tmem = nullptr;            // allocated by the first set_terrain to a non-flat source: normals, then held
-  double* normals = nullptr;       // [12][B] terrain_normals_kernel's estimate
+  void* tmem = nullptr;            // allocated by the first set_terrain / set_stance_terrain to a non-flat source: normals, then held
+  double* normals = nullptr;       // [12][B] terrain_normals_kernel's (MPC) or surface_normals_kernel's (QP) estimate
   uint32_t* held = nullptr;        // [N][B] the held pattern as a schedule (gait.horizon = 0), else NULL
 };
 
@@ -1005,6 +1041,21 @@ int tick_reset_impl(a1mpc_tick* t) {
   CK(cudaMemsetAsync(t->reset, 0, lb, h->stream));   // the EKF init of every robot supersedes a pending partial one
   t->first = true;
   t->pending = false;
+  return A1MPC_OK;
+}
+
+// the first non-flat terrain source of a tick: its normals [12][B] and, held_bytes > 0, the held pattern as a schedule
+int tick_terrain_alloc(a1mpc_tick* t, size_t held_bytes) {
+  if (t->tmem) return A1MPC_OK;
+  auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t nb = pad(12 * (size_t)t->B * sizeof(double));
+  if (cudaMalloc(&t->tmem, nb + held_bytes) != cudaSuccess) {
+    cudaGetLastError();
+    t->tmem = nullptr;
+    return fail(A1MPC_ENOMEM, "cudaMalloc failed");
+  }
+  t->normals = static_cast<double*>(t->tmem);
+  t->held = held_bytes ? reinterpret_cast<uint32_t*>(static_cast<char*>(t->tmem) + nb) : nullptr;
   return A1MPC_OK;
 }
 
@@ -1197,19 +1248,28 @@ int a1mpc_tick_set_terrain(a1mpc_tick* t, int source, const double* normals) {
   CK(cudaSetDevice(h->device));
   if (source == A1MPC_TERRAIN_GIVEN && !is_device_ptr(normals)) return fail(A1MPC_EINVAL, "the given normals must be device memory");
   const size_t lb = (size_t)t->B;
-  if (!t->tmem) {
-    auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t nb = pad(12 * lb * sizeof(double)), sb = t->sched ? 0 : (size_t)h->cfg.horizon * lb * 4;
-    if (cudaMalloc(&t->tmem, nb + sb) != cudaSuccess) {
-      cudaGetLastError();
-      t->tmem = nullptr;
-      return fail(A1MPC_ENOMEM, "cudaMalloc failed");
-    }
-    t->normals = static_cast<double*>(t->tmem);
-    t->held = sb ? reinterpret_cast<uint32_t*>(static_cast<char*>(t->tmem) + nb) : nullptr;
-  }
   int rc;
+  if ((rc = tick_terrain_alloc(t, t->sched ? 0 : (size_t)h->cfg.horizon * lb * 4))) return rc;
   if ((rc = ensure_capacity_ext(h, lb))) return rc;   // so that a run allocates nothing
+  t->terrain = source;
+  t->given = source == A1MPC_TERRAIN_GIVEN ? normals : nullptr;
+  return A1MPC_OK;
+}
+
+int a1mpc_tick_set_stance_terrain(a1mpc_tick* t, int source, const double* normals) {
+  if (!t) return fail(A1MPC_EINVAL, "null argument");
+  if (t->tp.mode != A1MPC_TICK_QP) return fail(A1MPC_EINVAL, "the stance terrain is for QP mode: an MPC-mode tick takes a1mpc_tick_set_terrain");
+  if (source != A1MPC_TERRAIN_FLAT && source != A1MPC_TERRAIN_ESTIMATED && source != A1MPC_TERRAIN_GIVEN) return fail(A1MPC_EINVAL, "unknown terrain source");
+  if (source == A1MPC_TERRAIN_FLAT) {
+    t->terrain = source;
+    t->given = nullptr;
+    return A1MPC_OK;
+  }
+  if (source == A1MPC_TERRAIN_GIVEN && !normals) return fail(A1MPC_EINVAL, "A1MPC_TERRAIN_GIVEN needs a normals array");
+  CK(cudaSetDevice(t->h->device));
+  if (source == A1MPC_TERRAIN_GIVEN && !is_device_ptr(normals)) return fail(A1MPC_EINVAL, "the given normals must be device memory");
+  int rc;
+  if ((rc = tick_terrain_alloc(t, 0))) return rc;   // the estimate only: the stance QP needs no schedule and no _ext queues
   t->terrain = source;
   t->given = source == A1MPC_TERRAIN_GIVEN ? normals : nullptr;
   return A1MPC_OK;
@@ -1237,7 +1297,7 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
   if ((rc = st.begin())) return rc;
   if ((rc = ensure_capacity(h, B))) return rc;   // create sized the scratch and it only grows: no allocation here
   if (!mpc && (rc = ensure_lists(h, stance_scratch_bytes(B)))) return rc;
-  if ((t->sched || t->tmem) && (rc = ensure_capacity_ext(h, B))) return rc;
+  if ((t->sched || (mpc && t->tmem)) && (rc = ensure_capacity_ext(h, B))) return rc;
   const a1mpc_tick_params& tp = t->tp;
   // 1-3: orientation and command
   CK(tick_front_a_launch(B, dt, quat, gyro, acc, t->imu, t->rot, t->rz, t->x0, t->ia, t->ig, t->cmd, cmd, t->mode, t->kpl, mpc ? t->ref : nullptr,
@@ -1305,11 +1365,20 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
     // world-z pyramids, shift 1 as the schedule moves one step per tick (a1mpc_solve_batch_ext at horizon 20, where t->warm is NULL)
     if ((rc = t->sched ? enqueue_solve_ext(h, B, di, t->sched, nullptr, dout, t->warm, 1) : enqueue_solve(h, B, di, dout, t->warm, 0))) return rc;
   } else {
+    // a1mpc_tick_set_stance_terrain: the walking surface's normal (no terrain stage in QP mode) or the given normals, then the stance QP
+    // with them; FLAT: world z
+    const double* nrm = t->terrain == A1MPC_TERRAIN_GIVEN ? t->given : nullptr;
+    if (t->terrain == A1MPC_TERRAIN_ESTIMATED) {
+      surface_normals_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->swing, t->x0 + 3 * lb, t->normals);
+      h->launches++;
+      CK(cudaGetLastError());
+      nrm = t->normals;
+    }
     double gains[9];
     for (int i = 0; i < 3; ++i) { gains[i] = tp.kd_linear[i]; gains[3 + i] = tp.kp_angular[i]; gains[6 + i] = tp.kd_angular[i]; }
     int nl = 0;
-    cudaError_t e = stance_qp_launch(h->sm_count, B, lb, t->x0, t->rot, t->rz, t->foot, t->contact, t->des, t->kpl, gains, h->cfg.mass, t->f_body,
-                                     t->status, nullptr, h->d_lists, h->stream, &nl);
+    cudaError_t e = stance_qp_launch(h->sm_count, B, lb, t->x0, t->rot, t->rz, t->foot, t->contact, t->des, t->kpl, gains, h->cfg.mass, nrm,
+                                     t->f_body, t->status, nullptr, h->d_lists, h->stream, &nl);
     if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("stance_qp kernels: ") + cudaGetErrorString(e));
     h->launches += nl;
   }

@@ -237,9 +237,16 @@ __global__ void __launch_bounds__(32 * Geo<NS, N>::TW) dense_solve_kernel(const 
 // compute_grf QP branch on one warp, for one robot: build the 12-variable QP of A1RobotControl.cpp:394-406, solve, rotate.
 // The inputs come from four arrays, rot_z / rot row-major and foot leg-major; the 12 forces go to f[(3 * leg + a) * fstride].
 // grf_qp_kernel (QP-major caller arrays) and stance_qp_kernel (the record of stance_pack_kernel, batch-major output) both run it.
-template <int NS>
+// EXT (stance_qp_ext_kernel): each stance foot's force is posed in its terrain frame T(n) = [e0 e1 e2] (terrain_col, the frame of the MPC's
+// _ext solve, so a foot gets the same pyramid in both modes): column (leg, b) of inertia_inv becomes [e_b ; Rz^T (p_leg x e_b)], the pyramid
+// and the 0 <= f_n <= 180 bounds of the unchanged solve act on the local forces, and the output is R^T T u_local.  R I is invariant under
+// the orthonormal T.  The normal of leg l is read at nin[(3 l + k) * nld] and normalised as pack_ext_kernel does; a stance foot's normal
+// that is not finite or has n_z <= 0 makes the QP NUMERICAL.  Ns: 12 doubles of the warp's shared memory that carry the unit normals
+// from the set-up lanes past the solve to the output lanes.
+template <int NS, bool EXT = false>
 __device__ __forceinline__ int grf_qp_body(const DevParams& P, Ctx<NS, 1>& c, double* Hs, double* Mi, int lane, int mask, const double* acc,
-                                           const double* rz, const double* R, const double* ft, double* f, size_t fstride) {
+                                           const double* rz, const double* R, const double* ft, double* f, size_t fstride,
+                                           const double* nin = nullptr, size_t nld = 0, double* Ns = nullptr) {
   using G = Geo<NS, 1>;
   constexpr int NV = G::NV;
   const double Qd[6] = {1.0, 1.0, 1.0, 400.0, 400.0, 100.0};  // A1RobotControl.cpp:11
@@ -251,15 +258,39 @@ __device__ __forceinline__ int grf_qp_body(const DevParams& P, Ctx<NS, 1>& c, do
   if (lane < 12) {
     const int leg = lane / 3, bb = lane - 3 * leg;
     const double rx = ft[3 * leg], ry = ft[3 * leg + 1], rzz = ft[3 * leg + 2];
-    const double s0 = (bb == 0) ? 0.0 : (bb == 1 ? -rzz : ry);
-    const double s1 = (bb == 0) ? rzz : (bb == 1 ? 0.0 : -rx);
-    const double s2 = (bb == 0) ? -ry : (bb == 1 ? rx : 0.0);
+    if (EXT) {
+      double e[3] = {bb == 0 ? 1.0 : 0.0, bb == 1 ? 1.0 : 0.0, bb == 2 ? 1.0 : 0.0};
+      bool nbad = false;
+      if ((mask >> leg) & 1) {   // a swing foot's normal is not read
+        double n[3] = {nin[(size_t)(3 * leg) * nld], nin[(size_t)(3 * leg + 1) * nld], nin[(size_t)(3 * leg + 2) * nld]};
+        const double inv = rsqrt(n[0] * n[0] + n[1] * n[1] + n[2] * n[2]);
+        n[0] *= inv; n[1] *= inv; n[2] *= inv;
+        if (!(n[2] > 0.0)) { nbad = true; n[0] = 0.0; n[1] = 0.0; n[2] = 1.0; }
+        Ns[lane] = bb == 0 ? n[0] : (bb == 1 ? n[1] : n[2]);
+        // every column with a constant index, then a select: a lane-dependent index would put n and the frame in local memory
+        double e0[3], e1[3], e2[3];
+        terrain_col(n, 0, e0); terrain_col(n, 1, e1); terrain_col(n, 2, e2);
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      Mi[a * 12 + lane] = (a == bb) ? 1.0 : 0.0;
-      Mi[(3 + a) * 12 + lane] = rz[0 * 3 + a] * s0 + rz[1 * 3 + a] * s1 + rz[2 * 3 + a] * s2;  // (Rz^T S)[a][bb]
+        for (int a = 0; a < 3; ++a) e[a] = bb == 0 ? e0[a] : (bb == 1 ? e1[a] : e2[a]);
+      }
+      const double s0 = ry * e[2] - rzz * e[1], s1 = rzz * e[0] - rx * e[2], s2 = rx * e[1] - ry * e[0];   // p x e_b
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        Mi[a * 12 + lane] = e[a];
+        Mi[(3 + a) * 12 + lane] = rz[0 * 3 + a] * s0 + rz[1 * 3 + a] * s1 + rz[2 * 3 + a] * s2;  // (Rz^T (p x e_b))[a]
+      }
+      bad = nbad;
+    } else {
+      const double s0 = (bb == 0) ? 0.0 : (bb == 1 ? -rzz : ry);
+      const double s1 = (bb == 0) ? rzz : (bb == 1 ? 0.0 : -rx);
+      const double s2 = (bb == 0) ? -ry : (bb == 1 ? rx : 0.0);
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        Mi[a * 12 + lane] = (a == bb) ? 1.0 : 0.0;
+        Mi[(3 + a) * 12 + lane] = rz[0 * 3 + a] * s0 + rz[1 * 3 + a] * s1 + rz[2 * 3 + a] * s2;  // (Rz^T S)[a][bb]
+      }
     }
-    bad = !(fabs(rx) < 1e300) || !(fabs(ry) < 1e300) || !(fabs(rzz) < 1e300);
+    bad = bad || !(fabs(rx) < 1e300) || !(fabs(ry) < 1e300) || !(fabs(rzz) < 1e300);
   }
   if (lane < 6) bad = bad || !(fabs(acc[lane]) < 1e300);
   bad = __any_sync(0xffffffffu, bad);
@@ -324,7 +355,14 @@ __device__ __forceinline__ int grf_qp_body(const DevParams& P, Ctx<NS, 1>& c, do
     for (int k = 0; k < 4; ++k)
       if (k < NS && leg_of[k] == lane && ((mask >> lane) & 1)) sfi = k;
     if (sfi >= 0) {
-      const double ux = c.vy[3 * sfi] * FSCALE, uy = c.vy[3 * sfi + 1] * FSCALE, uz = c.vy[3 * sfi + 2] * FSCALE;
+      double ux = c.vy[3 * sfi] * FSCALE, uy = c.vy[3 * sfi + 1] * FSCALE, uz = c.vy[3 * sfi + 2] * FSCALE;
+      if (EXT) {   // local -> world: T u
+        const double n[3] = {Ns[3 * lane], Ns[3 * lane + 1], Ns[3 * lane + 2]};
+        double e0[3], e1[3], e2[3];
+        terrain_col(n, 0, e0); terrain_col(n, 1, e1); terrain_col(n, 2, e2);
+        const double wx = e0[0] * ux + e1[0] * uy + e2[0] * uz, wy = e0[1] * ux + e1[1] * uy + e2[1] * uz, wz = e0[2] * ux + e1[2] * uy + e2[2] * uz;
+        ux = wx; uy = wy; uz = wz;
+      }
 #pragma unroll
       for (int a = 0; a < 3; ++a) fo[a] = R[a] * ux + R[3 + a] * uy + R[6 + a] * uz;
     }
@@ -456,6 +494,32 @@ __global__ void __launch_bounds__(32) stance_qp_kernel(const __grid_constant__ D
   }
 }
 
+// a1mpc_stance_qp_batch_ext: stance_qp_kernel with per-foot terrain normals [12][ld] (grf_qp_body<NS, true>); the unit normals are staged
+// in 12 doubles behind the inertia_inv scratch
+template <int NS>
+__global__ void __launch_bounds__(32) stance_qp_ext_kernel(const __grid_constant__ DevParams P, const double* __restrict__ rec,
+                                                           const uint32_t* __restrict__ contact, const int* __restrict__ list,
+                                                           const int* __restrict__ count, const double* __restrict__ normals,
+                                                           double* __restrict__ f_body, size_t ld, int32_t* __restrict__ status) {
+  using G = Geo<NS, 1>;
+  A1MPC_DYN_SMEM(smem);
+  const int lane = threadIdx.x;
+  Ctx<NS, 1> c(smem + G::TAB_DOUBLES, smem, lane);
+  double* Hs = smem + G::TAB_DOUBLES + G::WARP_DOUBLES;
+  double* Mi = Hs + DenseGeo<NS, 1>::HS;  // 6 x 12 inertia_inv scratch
+  double* Ns = Mi + 72;                   // 4 x 3 unit normals
+  const int nq = count[NS];
+#pragma unroll 1
+  for (int q = blockIdx.x; q < nq; q += gridDim.x) {
+    const int b = list[q];
+    const int mask = contact[b] & 15;
+    const double* r = rec + (size_t)b * STANCE_REC;
+    const int st = grf_qp_body<NS, true>(P, c, Hs, Mi, lane, mask, r, r + 6, r + 15, r + 24, f_body + b, ld, normals + b, ld, Ns);
+    if (lane == 0) status[b] = st;
+    __syncwarp();
+  }
+}
+
 // the QP constants of compute_grf (A1RobotControl.cpp:13-15); Q and R are literals of grf_qp_body
 inline DevParams grf_params() {
   DevParams P;
@@ -563,11 +627,18 @@ cudaError_t grf_qp_launch(int sm_count, int B, const double* root_acc, const dou
 
 template <int NS>
 static cudaError_t stance_launch_one(const DevParams& P, int sm_count, int B, const double* rec, const uint32_t* contact, const int* list,
-                                     const int* count, double* f_body, size_t ld, int32_t* status, cudaStream_t st) {
+                                     const int* count, const double* normals, double* f_body, size_t ld, int32_t* status, cudaStream_t st) {
+  int grid = B < sm_count * 16 ? B : sm_count * 16;
+  if (normals) {
+    const size_t smem = DenseGeo<NS, 1>::smem_bytes() + 84 * 8;
+    cudaError_t e = cudaFuncSetAttribute(stance_qp_ext_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    stance_qp_ext_kernel<NS><<<grid, 32, smem, st>>>(P, rec, contact, list + (size_t)(NS - 1) * B, count, normals, f_body, ld, status);
+    return cudaGetLastError();
+  }
   const size_t smem = DenseGeo<NS, 1>::smem_bytes() + 72 * 8;
   cudaError_t e = cudaFuncSetAttribute(stance_qp_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  int grid = B < sm_count * 16 ? B : sm_count * 16;
   stance_qp_kernel<NS><<<grid, 32, smem, st>>>(P, rec, contact, list + (size_t)(NS - 1) * B, count, f_body, ld, status);
   return cudaGetLastError();
 }
@@ -578,7 +649,8 @@ size_t stance_scratch_bytes(int B) { return stance_lists_bytes(B) + (size_t)B * 
 
 cudaError_t stance_qp_launch(int sm_count, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
                              const uint32_t* contact, const double* des, const double* kp_linear, const double* gains9, double mass,
-                             double* f_body, int32_t* status, double* root_acc, void* scratch, cudaStream_t st, int* nlaunch) {
+                             const double* normals, double* f_body, int32_t* status, double* root_acc, void* scratch, cudaStream_t st,
+                             int* nlaunch) {
   const DevParams P = grf_params();
   StanceGains G;
   for (int i = 0; i < 3; ++i) { G.kd_lin[i] = gains9[i]; G.kp_ang[i] = gains9[3 + i]; G.kd_ang[i] = gains9[6 + i]; }
@@ -590,10 +662,10 @@ cudaError_t stance_qp_launch(int sm_count, int B, size_t ld, const double* x0, c
   if (e != cudaSuccess) return e;
   stance_pack_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, ld, x0, rot, rot_z, foot, contact, des, kp_linear, G, rec, list, count, f_body, status,
                                                        root_acc);
-  if ((e = stance_launch_one<4>(P, sm_count, B, rec, contact, list, count, f_body, ld, status, st)) != cudaSuccess) return e;
-  if ((e = stance_launch_one<3>(P, sm_count, B, rec, contact, list, count, f_body, ld, status, st)) != cudaSuccess) return e;
-  if ((e = stance_launch_one<2>(P, sm_count, B, rec, contact, list, count, f_body, ld, status, st)) != cudaSuccess) return e;
-  if ((e = stance_launch_one<1>(P, sm_count, B, rec, contact, list, count, f_body, ld, status, st)) != cudaSuccess) return e;
+  if ((e = stance_launch_one<4>(P, sm_count, B, rec, contact, list, count, normals, f_body, ld, status, st)) != cudaSuccess) return e;
+  if ((e = stance_launch_one<3>(P, sm_count, B, rec, contact, list, count, normals, f_body, ld, status, st)) != cudaSuccess) return e;
+  if ((e = stance_launch_one<2>(P, sm_count, B, rec, contact, list, count, normals, f_body, ld, status, st)) != cudaSuccess) return e;
+  if ((e = stance_launch_one<1>(P, sm_count, B, rec, contact, list, count, normals, f_body, ld, status, st)) != cudaSuccess) return e;
   if (nlaunch) *nlaunch = 5;
   return cudaGetLastError();
 }

@@ -46,11 +46,13 @@ cudaError_t dense_solve_launch(const DevParams& P, int sm_count, int B, const do
 cudaError_t grf_qp_launch(int sm_count, int B, const double* root_acc, const double* rot_z, const double* rot, const double* foot,
                           const uint32_t* contact, double* f_body, int32_t* status, int* scratch, cudaStream_t st, int* nlaunch);
 // the same QP with the PD law in front of it, batch-major arrays with leading dimension ld (a1mpc_stance_qp_batch);
-// gains9 = kd_linear, kp_angular, kd_angular (host); scratch: stance_scratch_bytes(B) bytes of device memory
+// gains9 = kd_linear, kp_angular, kd_angular (host); scratch: stance_scratch_bytes(B) bytes of device memory.  normals [12][ld] (device)
+// poses each stance foot's pyramid on its terrain normal (a1mpc_stance_qp_batch_ext); NULL: world z
 size_t stance_scratch_bytes(int B);
 cudaError_t stance_qp_launch(int sm_count, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
                              const uint32_t* contact, const double* des, const double* kp_linear, const double* gains9, double mass,
-                             double* f_body, int32_t* status, double* root_acc, void* scratch, cudaStream_t st, int* nlaunch);
+                             const double* normals, double* f_body, int32_t* status, double* root_acc, void* scratch, cudaStream_t st,
+                             int* nlaunch);
 
 // orientation and command stages (a1mpc_command.cu, kernels in a1mpc_command.cuh), thread per robot on the stream
 size_t imu_state_doubles();       // per robot

@@ -283,6 +283,23 @@ __global__ void terrain_pitch_kernel(int B, double* __restrict__ state, int adap
 constexpr double SW_TILT_MAX = 0.5;                                                   // the angle clip of A1RobotControl.cpp:347-352
 constexpr double SW_TILT_SIN = 0.479425538604203, SW_TILT_COS = 0.8775825618903728;   // sin 0.5, cos 0.5
 
+// the walking surface's unit normal in the world frame from the swing state of the robot that starts at s and its root_pos z: the
+// fitted plane's own normal (-a1, -a2, 1) / |.|, its tilt clipped to 0.5 rad about the same horizontal axis, e_z while z <= 0.1
+__device__ __forceinline__ void sw_surface_normal(const double* s, size_t ld, double root_z, double (&n)[3]) {
+  double a[3];
+  sw_plane(s, ld, a);
+  n[0] = 0.0; n[1] = 0.0; n[2] = 1.0;
+  if (root_z > 0.1) {
+    if (acos(1.0 / sqrt(a[1] * a[1] + a[2] * a[2] + 1.0)) > SW_TILT_MAX) {   // terrain_body's angle before the filter
+      const double h = SW_TILT_SIN / sqrt(a[1] * a[1] + a[2] * a[2]);
+      n[0] = -a[1] * h; n[1] = -a[2] * h; n[2] = SW_TILT_COS;
+    } else {
+      const double inv = 1.0 / sqrt(a[1] * a[1] + a[2] * a[2] + 1.0);
+      n[0] = -a[1] * inv; n[1] = -a[2] * inv; n[2] = inv;
+    }
+  }
+}
+
 // terrain_pitch_kernel's stage, and the walking surface's unit normal in the world frame for the friction pyramids of the solve:
 // normals [12][B], the same for all four feet.  The plane is fitted in the frame of foot_pos_recent_contact (world axes), so its normal
 // is (-a1, -a2, 1) / |.|; a tilt beyond 0.5 rad is clipped to 0.5 about the same horizontal axis, and while the body is low (the filter
@@ -295,18 +312,8 @@ __global__ void terrain_normals_kernel(int B, double* __restrict__ state, int ad
   if (b >= B) return;
   const size_t ld = (size_t)B;
   terrain_body(b, B, state, adapt, root_pos, ref, ref_ld, pitch);
-  double a[3];
-  sw_plane(state + b, ld, a);
-  double n[3] = {0.0, 0.0, 1.0};
-  if (root_pos[2 * ld + b] > 0.1) {
-    if (acos(1.0 / sqrt(a[1] * a[1] + a[2] * a[2] + 1.0)) > SW_TILT_MAX) {   // terrain_body's angle before the filter
-      const double h = SW_TILT_SIN / sqrt(a[1] * a[1] + a[2] * a[2]);
-      n[0] = -a[1] * h; n[1] = -a[2] * h; n[2] = SW_TILT_COS;
-    } else {
-      const double inv = 1.0 / sqrt(a[1] * a[1] + a[2] * a[2] + 1.0);
-      n[0] = -a[1] * inv; n[1] = -a[2] * inv; n[2] = inv;
-    }
-  }
+  double n[3];
+  sw_surface_normal(state + b, ld, root_pos[2 * ld + b], n);
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -315,6 +322,21 @@ __global__ void terrain_normals_kernel(int B, double* __restrict__ state, int ad
     const uint32_t c = contacts[b];
     for (int k = 0; k < N; ++k) sched[(size_t)k * ld + b] = c;
   }
+}
+
+// the walking surface's normal of terrain_normals_kernel without the terrain stage, thread per robot: the ESTIMATED source of a QP-mode tick
+// (the reference adapts to terrain only in MPC mode, so terrain_angle_filter and ref stay as they are).  It only reads the swing state,
+// whose recent-contact points the swing stage records in both modes; normals [12][B], the same for all four feet.
+__global__ void surface_normals_kernel(int B, const double* __restrict__ state, const double* __restrict__ root_pos, double* __restrict__ normals) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const size_t ld = (size_t)B;
+  double n[3];
+  sw_surface_normal(state + b, ld, root_pos[2 * ld + b], n);
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) normals[(size_t)(3 * i + k) * ld + b] = n[k];
 }
 
 }  // namespace a1mpc

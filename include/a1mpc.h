@@ -241,6 +241,18 @@ int  a1mpc_grf_qp_batch(a1mpc_handle* h, int B, const double* root_acc, const do
 int  a1mpc_stance_qp_batch(a1mpc_handle* h, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
                            const uint32_t* contact, const double* des, const double* kp_linear, const double* kd_linear,
                            const double* kp_angular, const double* kd_angular, double* f_body, int32_t* status, double* root_acc);
+/* a1mpc_stance_qp_batch with each stance foot's friction pyramid on the walking surface rather than world z.  normals [12][ld]: per foot
+ * (leg-major, x y z), world frame, host or device like the other batch arrays; the engine normalises them as a1mpc_solve_batch_ext does.
+ * Each stance foot's force is solved in the foot's terrain frame T(n) (the rotation about z x n that takes world z to n, the frame of the
+ * a1mpc_solve_batch_ext pyramids, so a foot gets the same pyramid in QP and MPC mode): |t_x|, |t_y| <= 0.7 f_n and 0 <= f_n <= 180 act on
+ * T(n)^T f_world.  The QP is the same in the world forces, H = R I + M^T Q M, g = -M^T Q root_acc.  f_body is R^T T u_local.
+ * A stance foot whose normal is not finite, or has n_z <= 0 after normalisation, makes the robot A1MPC_STATUS_NUMERICAL with zero forces;
+ * a swing foot's normal is not read.  All-e_z normals give exactly what a1mpc_stance_qp_batch gives; normals == NULL is that call.
+ * fp64 whatever cfg.precision says. */
+int  a1mpc_stance_qp_batch_ext(a1mpc_handle* h, int B, size_t ld, const double* x0, const double* rot, const double* rot_z, const double* foot,
+                               const uint32_t* contact, const double* des, const double* kp_linear, const double* kd_linear,
+                               const double* kp_angular, const double* kd_angular, const double* normals, double* f_body, int32_t* status,
+                               double* root_acc);
 
 /* ---- the step right after the path (SURVEY 8f.1): A1RobotControl::compute_joint_torques ------------- */
 /* A1RobotControl.cpp:289-319, batched, batch-major SoA like a1mpc_solve_batch (ld = B), host or device pointers:
@@ -345,6 +357,10 @@ int  a1mpc_update_plan_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp
  *                              (-a1, -a2, 1) / |.| (z = a0 + a1 x + a2 y in the frame of foot_pos_recent_contact, which has world
  *                              axes), its tilt clipped to 0.5 rad about the same horizontal axis, and e_z while root_pos z <= 0.1;
  *                              so n_z >= cos 0.5 > 0.  It advances the same filter: a chain calls one of the two, never both.
+ *   a1mpc_surface_normals_batch  the normals of a1mpc_terrain_normals_batch, bit for bit, without its terrain stage: swing_state (device
+ *                              memory) is only read, no filter advances and no ref is written.  The reference adapts to terrain only in
+ *                              MPC mode, so this is the walking surface of a QP-mode chain (a1mpc_tick_set_stance_terrain's ESTIMATED
+ *                              source, staged).  root_pos [3][B] in, normals [12][B] out, host or device.
  */
 size_t a1mpc_swing_bytes(int B);
 int  a1mpc_swing_init_batch(a1mpc_handle* h, int B, void* swing_state);
@@ -356,6 +372,7 @@ int  a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int us
                                double* terrain_pitch);
 int  a1mpc_terrain_normals_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref,
                                  size_t ref_ld, double* terrain_pitch, double* normals);
+int  a1mpc_surface_normals_batch(a1mpc_handle* h, int B, const void* swing_state, const double* root_pos, double* normals);
 
 /* ---- the first two stages of a control tick: the adapters' orientation and command stages ---------------------------------
  * Together with the stages above they let a whole tick run from raw sensor arrays on device pointers.  One thread per robot;
@@ -445,7 +462,7 @@ int  a1mpc_command_batch(a1mpc_handle* h, int B, void* cmd_state, double dt, con
  *       feet the torque stage treats as stance), world-z friction pyramids (no normals).  Like a1mpc_solve_batch_ext it does not take
  *       part in the fused collect.  The schedule stays inside the tick.
  *     Either way the friction pyramids stand on world z unless a1mpc_tick_set_terrain chose another source (below).
- *     A1MPC_TICK_QP: a1mpc_stance_qp_batch.
+ *     A1MPC_TICK_QP: a1mpc_stance_qp_batch (world-z pyramids unless a1mpc_tick_set_stance_terrain chose another source, below).
  *   8 joint torques.
  * The arrays connect as in a hand-built chain of those entry points: x0 rows 3-5 / 9-11 are the EKF's estimate (zero until its first
  * update), update_plan's root_lin_vel_d is ref row 5 (MPC) or des row 6 (QP), and in MPC mode the command stage reads ref row 1 back, so
@@ -516,12 +533,24 @@ int  a1mpc_tick_reset_robots(a1mpc_tick* t, const uint8_t* mask);
  * source between runs needs no clean-up: the warm slots of the held-pattern solve and of the _ext solve read each other as "no guess".
  * The first call to a non-flat source allocates the tick's normals and held schedule and sizes the handle's scratch (it may
  * synchronise); after it a run on device arrays still allocates nothing and does not synchronise.  a1mpc_tick_reset and
- * a1mpc_tick_reset_robots keep the source.  A1MPC_EINVAL: a NULL tick, an unknown source, a non-flat source in QP mode (the stance QP
- * keeps its world-z pyramid) or on a handle with non-isotropic r, GIVEN with a NULL or host pointer. */
+ * a1mpc_tick_reset_robots keep the source.  A1MPC_EINVAL: a NULL tick, an unknown source, a non-flat source in QP mode (a QP-mode tick
+ * takes a1mpc_tick_set_stance_terrain below) or on a handle with non-isotropic r, GIVEN with a NULL or host pointer. */
 #define A1MPC_TERRAIN_FLAT      0
 #define A1MPC_TERRAIN_ESTIMATED 1
 #define A1MPC_TERRAIN_GIVEN     2
 int  a1mpc_tick_set_terrain(a1mpc_tick* t, int source, const double* normals);
+/* Where a QP-mode tick's stance friction pyramids stand (stage 7), with the sources of a1mpc_tick_set_terrain:
+ *   A1MPC_TERRAIN_FLAT       world z, the default: the tick as if this call had never been made (normals ignored).
+ *   A1MPC_TERRAIN_ESTIMATED  the walking surface's normal (a1mpc_surface_normals_batch) from the recent-contact points the swing stage
+ *                            records, the same for all four feet.
+ *   A1MPC_TERRAIN_GIVEN      normals [12][B]: a caller-owned DEVICE array (per foot, world frame, n_z > 0) that every later run reads at
+ *                            stage 7; the caller orders its writes before the run.
+ * With ESTIMATED or GIVEN, stage 7 is a1mpc_surface_normals_batch (ESTIMATED only) and then a1mpc_stance_qp_batch_ext with those normals.
+ * Stage 7 writes nothing else: the reference adapts to terrain only in MPC mode, so no terrain filter advances and des is untouched.  The
+ * first call to a non-flat source allocates the tick's normals (it may synchronise); after it a run on device arrays allocates nothing and
+ * does not synchronise.  a1mpc_tick_reset and a1mpc_tick_reset_robots keep the source.  A1MPC_EINVAL: a NULL tick, an MPC-mode tick (it
+ * takes a1mpc_tick_set_terrain), an unknown source, GIVEN with a NULL or host pointer. */
+int  a1mpc_tick_set_stance_terrain(a1mpc_tick* t, int source, const double* normals);
 int  a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out);
 int  a1mpc_tick_destroy(a1mpc_tick* t);
 
