@@ -22,7 +22,7 @@ EXPORTS = [
     "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_stance_qp_batch_ext", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
     "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_terrain_normals_batch", "a1mpc_surface_normals_batch",
     "a1mpc_imu_bytes", "a1mpc_imu_init_batch", "a1mpc_orientation_batch", "a1mpc_command_bytes", "a1mpc_command_init_batch", "a1mpc_command_batch",
-    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_set_terrain", "a1mpc_tick_set_stance_terrain", "a1mpc_tick_run", "a1mpc_tick_destroy",
+    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_set_terrain", "a1mpc_tick_set_stance_terrain", "a1mpc_tick_set_mpc_period", "a1mpc_plan_forces_batch", "a1mpc_tick_run", "a1mpc_tick_destroy",
     "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
@@ -81,6 +81,7 @@ def default_command_params(variant=VARIANT_GAZEBO):
 
 TICK_QP, TICK_MPC = 0, 1
 TERRAIN_FLAT, TERRAIN_ESTIMATED, TERRAIN_GIVEN = 0, 1, 2   # a1mpc_tick_set_terrain
+PLAYBACK_HOLD, PLAYBACK_PLAN = 0, 1                        # a1mpc_tick_set_mpc_period
 
 
 class TickParams(C.Structure):
@@ -195,6 +196,8 @@ def lib():
         l.a1mpc_tick_reset_robots.argtypes = [C.c_void_p, C.c_void_p]
         l.a1mpc_tick_set_terrain.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         l.a1mpc_tick_set_stance_terrain.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        l.a1mpc_tick_set_mpc_period.argtypes = [C.c_void_p, C.c_int, C.c_int]
+        l.a1mpc_plan_forces_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 4
         l.a1mpc_tick_run.argtypes = [C.c_void_p, C.c_double, C.POINTER(TickInputs), C.POINTER(TickOutputs)]
         l.a1mpc_tick_destroy.argtypes = [C.c_void_p]
         l.a1mpc_gen_states.argtypes = [C.c_int, C.c_uint64, C.c_int] + [C.c_void_p] * 5
@@ -293,7 +296,8 @@ class Tick:
     the reference does; the engine's horizon runs the scheduled tick, whose solve sees the gait's planned contacts over the horizon (step 0
     the swing stage's contacts) and does not take part in the fused collect.  Any other value is rejected; QP mode ignores it.
     set_terrain picks where the MPC solve's friction pyramids stand: world z (the default), the estimated walking surface or the caller's
-    normals; set_stance_terrain does the same for the QP-mode stance QP."""
+    normals; set_stance_terrain does the same for the QP-mode stance QP.  set_mpc_period runs the MPC solve of each robot on every k-th
+    run only, staggered across the batch."""
 
     _SHAPES = dict(quat=(4,), gyro=(3,), acc=(3,), joint_pos=(12,), joint_vel=(12,), foot_force=(4,), cmd=(7,), gait_counter_speed=(4,))
 
@@ -357,6 +361,12 @@ class Tick:
         TERRAIN_ESTIMATED (the walking surface fitted through the recent-contact points) or TERRAIN_GIVEN with normals_ptr a device pointer to
         [12][B] float64 per-foot normals, read by every later run.  QP mode only"""
         _check(lib().a1mpc_tick_set_stance_terrain(self.t, int(source), normals_ptr or None))
+
+    def set_mpc_period(self, period, playback=PLAYBACK_PLAN):
+        """a1mpc_tick_set_mpc_period: robot b solves the MPC on its runs n with n == 0 or n % period == b % period (period 1..N, MPC mode);
+        on its other runs PLAYBACK_PLAN applies the step of its last solve's plan that belongs to the run, rotated by this run's rot, and
+        PLAYBACK_HOLD keeps the forces and status of its last solve.  Every robot solves on the next run"""
+        _check(lib().a1mpc_tick_set_mpc_period(self.t, int(period), int(playback)))
 
     def close(self):
         """a1mpc_tick_destroy; a tick whose Engine is closed has already been destroyed by Engine.close"""
@@ -623,6 +633,18 @@ class Engine:
         normals = np.zeros((12, B))
         _check(lib().a1mpc_surface_normals_batch(self.h, B, swing, _p(pos), _p(normals)))
         return normals
+
+    def plan_forces(self, rot, u_full, step, f_body=None):
+        """a1mpc_plan_forces_batch on host arrays: rot [9][B], u_full [12N][B], step [B] -> f_body [12][B] (a copy of the given f_body, or
+        zeros, where step is 0; R^T of plan step `step` where 0 < step < N; zero forces where step >= N)"""
+        B = np.shape(step)[0]
+        r = np.ascontiguousarray(rot, dtype=np.float64); u = np.ascontiguousarray(u_full, dtype=np.float64)
+        s = np.ascontiguousarray(step, dtype=np.uint32)
+        f = np.array(f_body, dtype=np.float64, order="C") if f_body is not None else np.zeros((12, B))
+        if r.shape != (9, B) or u.shape != (12 * self.cfg.horizon, B) or f.shape != (12, B):
+            raise ValueError("rot must be [9][B], u_full [12N][B] and f_body [12][B]")
+        _check(lib().a1mpc_plan_forces_batch(self.h, B, _p(r), _p(u), _p(s), _p(f)))
+        return f
 
     def imu_alloc(self, B):
         """device-resident IMU filter state of B robots (a1mpc_imu_bytes), initialised by a1mpc_imu_init_batch; bound to this B"""

@@ -268,14 +268,18 @@ int peer_signal(a1mpc_handle* h, int B) {
   return A1MPC_OK;
 }
 
-int enqueue_solve(a1mpc_handle* h, int B, const DevInputs& din, const DevOutputs& dout_in, uint32_t* warm = nullptr, int shift = 0) {
+// runs: the multi-rate tick's run counters (a1mpc_tick_set_mpc_period), whose robots that are not due this run the pack kernel skips;
+// such a solve does not take part in the fused collect
+int enqueue_solve(a1mpc_handle* h, int B, const DevInputs& din, const DevOutputs& dout_in, uint32_t* warm = nullptr, int shift = 0,
+                  const uint32_t* runs = nullptr, int period = 1) {
   DevOutputs dout = dout_in;
-  attach_peers(h, B, dout);
+  attach_peers(h, runs ? -1 : B, dout);
 #if A1MPC_TIMELINE
   dout.tl = h->tl;
 #endif
   CK(cudaMemsetAsync(h->d_count, 0, 16 * sizeof(int), h->stream));
-  pack_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(din, B, h->d_rec, (int)h->cap, h->d_count, dout, h->cfg.horizon);
+  if (runs) pack_due_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(din, B, h->d_rec, (int)h->cap, h->d_count, dout, h->cfg.horizon, runs, period);
+  else pack_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(din, B, h->d_rec, (int)h->cap, h->d_count, dout, h->cfg.horizon);
   h->launches++;
   CK(cudaEventRecord(h->ev_fork, h->stream));
   const int N = h->cfg.horizon;
@@ -298,12 +302,13 @@ int enqueue_solve(a1mpc_handle* h, int B, const DevInputs& din, const DevOutputs
   }
   if (h->prof_on && h->prof_n < h->prof_cap) h->prof_n++;
   CK(cudaGetLastError());
+  if (runs) return A1MPC_OK;
   return peer_signal(h, B);   // fused collect: publish this call's step number to every rank (no-op when not connected)
 }
 
 // the same on a schedule (dsched) and / or terrain normals (dnorm): a1mpc_solve_batch_ext and _ext_warm
 int enqueue_solve_ext(a1mpc_handle* h, int B, const DevInputs& di, const uint32_t* dsched, const double* dnorm, const DevOutputs& dout_in,
-                      uint32_t* warm, int shift) {
+                      uint32_t* warm, int shift, const uint32_t* runs = nullptr, int period = 1) {
   const int N = h->cfg.horizon;
   int rc;
   if ((rc = ensure_capacity_ext(h, B))) return rc;
@@ -314,11 +319,15 @@ int enqueue_solve_ext(a1mpc_handle* h, int B, const DevInputs& di, const uint32_
 #endif
   CK(cudaMemsetAsync(h->d_count, 0, 16 * sizeof(int), h->stream));
   if (warm) {   // robots without any contact are answered by the pack kernel and store no guess
-    warm_forget_no_contact_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, B, warm, N);
+    if (runs) warm_forget_no_contact_due_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, B, warm, N, runs, period);
+    else warm_forget_no_contact_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, B, warm, N);
     h->launches++;
   }
   if (h->ext_compact && dsched) {
-    pack_ext2_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, (int)h->cap_ext, h->d_count, dout, N);
+    if (runs)
+      pack_ext2_due_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, (int)h->cap_ext, h->d_count, dout, N, runs, period);
+    else
+      pack_ext2_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, (int)h->cap_ext, h->d_count, dout, N);
     const double* rec2 = h->d_rec_ext + h->cap_ext * REC_EXT_DOUBLES;
     if (warm) {
       ext_warm_launch(h->cls_ext_warm, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout, warm, shift);
@@ -329,7 +338,8 @@ int enqueue_solve_ext(a1mpc_handle* h, int B, const DevInputs& di, const uint32_
     }
     h->launches += 3;
   } else {
-    pack_ext_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, h->d_count, dout, N);
+    if (runs) pack_ext_due_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, h->d_count, dout, N, runs, period);
+    else pack_ext_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(di, dsched, dnorm, B, h->d_rec_ext, h->d_count, dout, N);
     if (warm) ext_warm_launch(h->cls_ext_warm, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout, warm, shift);
     else ext_launch(N, h->cls_ext, h->stream, B, h->P, h->d_rec_ext, h->d_count, dout);
     h->launches += 2;
@@ -918,6 +928,21 @@ int a1mpc_surface_normals_batch(a1mpc_handle* h, int B, const void* swing_state,
 // ---- orientation and command stages (the adapters' IMU / pose callbacks and main_update's front half) ------------------------
 size_t a1mpc_imu_bytes(int B) { return B > 0 ? (size_t)B * imu_state_doubles() * sizeof(double) : 0; }
 
+int a1mpc_plan_forces_batch(a1mpc_handle* h, int B, const double* rot, const double* u_full, const uint32_t* step, double* f_body) {
+  if (!h || !rot || !u_full || !step || !f_body) return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  const int N = h->cfg.horizon;
+  CK(cudaSetDevice(h->device));
+  Stage st(h, B);
+  st.in(rot, 9); st.in(u_full, 12 * (size_t)N); st.in(step, 1); st.inout(f_body, 12);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  plan_forces_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, N, rot, u_full, step, f_body);
+  h->launches++;
+  CK(cudaGetLastError());
+  return st.finish();
+}
+
 int a1mpc_imu_init_batch(a1mpc_handle* h, int B, void* imu_state) {
   if (!h || !imu_state) return fail(A1MPC_EINVAL, "null argument");
   if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
@@ -1016,6 +1041,12 @@ struct a1mpc_tick {
   void* tmem = nullptr;            // allocated by the first set_terrain / set_stance_terrain to a non-flat source: normals, then held
   double* normals = nullptr;       // [12][B] terrain_normals_kernel's (MPC) or surface_normals_kernel's (QP) estimate
   uint32_t* held = nullptr;        // [N][B] the held pattern as a schedule (gait.horizon = 0), else NULL
+  // the MPC period (a1mpc_tick_set_mpc_period); rmem and plan are allocated by the first call that needs them
+  int period = 1;
+  int playback = A1MPC_PLAYBACK_HOLD;
+  void* rmem = nullptr;            // runs [B] (n_b), then since [B] (j_b)
+  uint32_t *runs = nullptr, *since = nullptr;
+  double* plan = nullptr;          // [12 N][B] each robot's u_full of its last solve (A1MPC_PLAYBACK_PLAN)
 };
 
 namespace {
@@ -1039,6 +1070,7 @@ int tick_reset_impl(a1mpc_tick* t) {
   CK(cudaGetLastError());
   if (t->warm) CK(cudaMemsetAsync(t->warm, 0, a1mpc_warm_bytes(h, B), h->stream));
   CK(cudaMemsetAsync(t->reset, 0, lb, h->stream));   // the EKF init of every robot supersedes a pending partial one
+  if (t->rmem) CK(cudaMemsetAsync(t->rmem, 0, 2 * lb * sizeof(uint32_t), h->stream));   // every robot solves on the next run
   t->first = true;
   t->pending = false;
   return A1MPC_OK;
@@ -1226,6 +1258,10 @@ int a1mpc_tick_reset_robots(a1mpc_tick* t, const uint8_t* mask) {
                                                                     t->tp.mode == A1MPC_TICK_MPC ? t->ref : nullptr, t->swing, t->warm,
                                                                     WARM_HDR + 4 * h->cfg.horizon, flag ? t->reset : nullptr);
   h->launches++;
+  if (t->rmem) {   // a period > 1 has been set: the masked robots solve on their next run
+    tick_rate_reset_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, mask, t->runs, t->since);
+    h->launches++;
+  }
   CK(cudaGetLastError());
   t->pending = t->pending || flag;
   return st.finish();
@@ -1272,6 +1308,38 @@ int a1mpc_tick_set_stance_terrain(a1mpc_tick* t, int source, const double* norma
   if ((rc = tick_terrain_alloc(t, 0))) return rc;   // the estimate only: the stance QP needs no schedule and no _ext queues
   t->terrain = source;
   t->given = source == A1MPC_TERRAIN_GIVEN ? normals : nullptr;
+  return A1MPC_OK;
+}
+
+int a1mpc_tick_set_mpc_period(a1mpc_tick* t, int period, int playback) {
+  if (!t) return fail(A1MPC_EINVAL, "null argument");
+  if (t->tp.mode != A1MPC_TICK_MPC) return fail(A1MPC_EINVAL, "the MPC period is for MPC mode: the QP-mode stance QP runs on every run");
+  a1mpc_handle* h = t->h;
+  const int N = h->cfg.horizon;
+  if (period < 1 || period > N) return fail(A1MPC_EINVAL, "period must run from 1 to the handle's horizon N = " + std::to_string(N));
+  if (playback != A1MPC_PLAYBACK_HOLD && playback != A1MPC_PLAYBACK_PLAN) return fail(A1MPC_EINVAL, "unknown playback");
+  CK(cudaSetDevice(h->device));
+  const size_t lb = (size_t)t->B;
+  if (period > 1 && !t->rmem) {
+    if (cudaMalloc(&t->rmem, 2 * lb * sizeof(uint32_t)) != cudaSuccess) {
+      cudaGetLastError();
+      t->rmem = nullptr;
+      return fail(A1MPC_ENOMEM, "cudaMalloc failed");
+    }
+    t->runs = static_cast<uint32_t*>(t->rmem);
+    t->since = t->runs + lb;
+  }
+  if (period > 1 && playback == A1MPC_PLAYBACK_PLAN && !t->plan) {
+    if (cudaMalloc(&t->plan, 12 * (size_t)N * lb * sizeof(double)) != cudaSuccess) {
+      cudaGetLastError();
+      t->plan = nullptr;
+      return fail(A1MPC_ENOMEM, "cudaMalloc failed");
+    }
+  }
+  // every robot solves on the next run: so the plan is written before it is read, and j_b stays below the new period
+  if (t->rmem) CK(cudaMemsetAsync(t->rmem, 0, 2 * lb * sizeof(uint32_t), h->stream));
+  t->period = period;
+  t->playback = playback;
   return A1MPC_OK;
 }
 
@@ -1342,7 +1410,11 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
   }
   t->first = false;
   t->pending = false;
-  // 7: terrain pitch and the MPC solve, or the stance QP
+  // 7: terrain pitch and the MPC solve, or the stance QP.  A multi-rate tick (period > 1) solves the robots that are due this run
+  // (the pack kernels skip the others), the scheduled tick with shift = period as a due robot's stored faces are `period` schedule
+  // steps old; then tick_rate_kernel advances the counters and, with a plan, plays it back for the others.
+  const uint32_t* runs = t->period > 1 ? t->runs : nullptr;
+  double* plan = runs && t->playback == A1MPC_PLAYBACK_PLAN ? t->plan : nullptr;
   if (mpc && t->terrain != A1MPC_TERRAIN_FLAT) {
     // the same stage plus the estimated normals (and the held pattern as a schedule), then the solve of a1mpc_solve_batch_ext_warm
     // with normals: shift 1 on the scheduled tick's schedule, shift 0 on the held one (a1mpc_solve_batch_ext at horizon 20)
@@ -1351,19 +1423,22 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
     h->launches++;
     CK(cudaGetLastError());
     const DevInputs di{t->x0, t->rot, t->foot, t->ref, t->contact, lb, 0};
-    const DevOutputs dout{t->f_body, t->status, nullptr, nullptr, lb, 0};
+    const DevOutputs dout{t->f_body, t->status, nullptr, plan, lb, 0};
     const double* nrm = t->terrain == A1MPC_TERRAIN_GIVEN ? t->given : t->normals;
-    if ((rc = t->sched ? enqueue_solve_ext(h, B, di, t->sched, nrm, dout, t->warm, 1) : enqueue_solve_ext(h, B, di, t->held, nrm, dout, t->warm, 0)))
+    if ((rc = t->sched ? enqueue_solve_ext(h, B, di, t->sched, nrm, dout, t->warm, t->period, runs, t->period)
+                       : enqueue_solve_ext(h, B, di, t->held, nrm, dout, t->warm, 0, runs, t->period)))
       return rc;
   } else if (mpc) {
     terrain_pitch_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->swing, tp.use_terrain_adapt ? 1 : 0, t->x0 + 3 * lb, t->ref, lb, nullptr);
     h->launches++;
     CK(cudaGetLastError());
     const DevInputs di{t->x0, t->rot, t->foot, t->ref, t->contact, lb, 0};
-    const DevOutputs dout{t->f_body, t->status, nullptr, nullptr, lb, 0};
+    const DevOutputs dout{t->f_body, t->status, nullptr, plan, lb, 0};
     // held pattern: a1mpc_solve_batch_warm, shift 0 (cold at horizon 20).  Scheduled: a1mpc_solve_batch_ext_warm on the schedule with
     // world-z pyramids, shift 1 as the schedule moves one step per tick (a1mpc_solve_batch_ext at horizon 20, where t->warm is NULL)
-    if ((rc = t->sched ? enqueue_solve_ext(h, B, di, t->sched, nullptr, dout, t->warm, 1) : enqueue_solve(h, B, di, dout, t->warm, 0))) return rc;
+    if ((rc = t->sched ? enqueue_solve_ext(h, B, di, t->sched, nullptr, dout, t->warm, t->period, runs, t->period)
+                       : enqueue_solve(h, B, di, dout, t->warm, 0, runs, t->period)))
+      return rc;
   } else {
     // a1mpc_tick_set_stance_terrain: the walking surface's normal (no terrain stage in QP mode) or the given normals, then the stance QP
     // with them; FLAT: world z
@@ -1381,6 +1456,11 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
                                      t->f_body, t->status, nullptr, h->d_lists, h->stream, &nl);
     if (e != cudaSuccess) return fail(A1MPC_ECUDA, std::string("stance_qp kernels: ") + cudaGetErrorString(e));
     h->launches += nl;
+  }
+  if (runs) {
+    tick_rate_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, t->period, h->cfg.horizon, t->runs, t->since, t->rot, plan, t->f_body);
+    h->launches++;
+    CK(cudaGetLastError());
   }
   // 8: joint torques
   {
@@ -1406,6 +1486,8 @@ int a1mpc_tick_destroy(a1mpc_tick* t) {
   cudaStreamSynchronize(t->h->stream);
   if (t->mem) cudaFree(t->mem);
   if (t->tmem) cudaFree(t->tmem);
+  if (t->rmem) cudaFree(t->rmem);
+  if (t->plan) cudaFree(t->plan);
   delete t;
   return A1MPC_OK;
 }

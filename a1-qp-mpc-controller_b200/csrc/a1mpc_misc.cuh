@@ -99,12 +99,56 @@ __global__ void pack_ext_kernel(DevInputs in, const uint32_t* __restrict__ sched
   }
 }
 
+// pack_ext_kernel's body for its masked variant (pack_ext_due_kernel).  pack_ext_kernel keeps its own inline copy: calling this
+// function from it reorders its SASS.
+__device__ __forceinline__ void pack_ext_one(const DevInputs& in, const uint32_t* __restrict__ sched, const double* __restrict__ normals, int b,
+                                             double* __restrict__ rec, int* __restrict__ count, const DevOutputs& out, int horizon) {
+  unsigned long long s0 = 0ull, s1 = 0ull;
+  for (int st = 0; st < horizon; ++st) {
+    const unsigned long long m = (sched ? sched[(size_t)st * in.ld + b] : in.contact[b]) & 15u;
+    if (st < 16) s0 |= m << (4 * st);
+    else s1 |= m << (4 * (st - 16));
+  }
+  if (s0 == 0ull && s1 == 0ull) {
+    st_zero_forces(out, b);
+    out.status[b] = A1MPC_STATUS_NO_CONTACT;
+    if (out.iters) out.iters[b] = 0;
+    if (out.u_full)
+      for (int k = 0; k < 12 * horizon; ++k) st_out(out.u_full, (size_t)k * out.ld + b, 0.0, out.f32);
+    return;
+  }
+  const int slot = atomicAdd(&count[5], 1);
+  double* r = rec + (size_t)slot * REC_EXT_DOUBLES;
+#pragma unroll
+  for (int k = 0; k < 12; ++k) r[k] = ld_in(in.x0, (size_t)k * in.ld + b, in.f32);
+#pragma unroll
+  for (int k = 0; k < 9; ++k) r[12 + k] = ld_in(in.rot, (size_t)k * in.ld + b, in.f32);
+#pragma unroll
+  for (int k = 0; k < 12; ++k) r[21 + k] = ld_in(in.foot, (size_t)k * in.ld + b, in.f32);
+#pragma unroll
+  for (int k = 0; k < 9; ++k) r[33 + k] = ld_in(in.ref, (size_t)k * in.ld + b, in.f32);
+  r[42] = __hiloint2double((int)(s0 & 15ull), b);
+  r[43] = 0.0;
+  r[44] = __longlong_as_double((long long)s0);
+  r[45] = __longlong_as_double((long long)s1);
+  for (int leg = 0; leg < 4; ++leg) {
+    double nx = 0.0, ny = 0.0, nz = 1.0;
+    if (normals) {
+      nx = ld_in(normals, (size_t)(3 * leg) * in.ld + b, in.f32); ny = ld_in(normals, (size_t)(3 * leg + 1) * in.ld + b, in.f32); nz = ld_in(normals, (size_t)(3 * leg + 2) * in.ld + b, in.f32);
+      const double inv = rsqrt(nx * nx + ny * ny + nz * nz);
+      nx *= inv; ny *= inv; nz *= inv;
+      // a terrain normal must point out of the ground (nz > 0, include/a1mpc.h): anything else is poisoned here and comes back as
+      // A1MPC_STATUS_NUMERICAL with zero forces from the solve kernel's input check instead of being clamped silently
+      if (!(nz > 0.0)) { nx = ny = nz = __longlong_as_double(0x7ff8000000000000ll); }
+    }
+    r[46 + 3 * leg] = nx; r[47 + 3 * leg] = ny; r[48 + 3 * leg] = nz;
+  }
+}
+
 // pack kernel of the extended path with the compacted class (A1MPC_EXT_COMPACT): schedules with exactly two stance feet in every
 // horizon step go to queue 6 (records behind the first `cap` records), everything else to queue 5 as in pack_ext_kernel
-__global__ void pack_ext2_kernel(DevInputs in, const uint32_t* __restrict__ sched, const double* __restrict__ normals, int B,
-                                 double* __restrict__ rec, int cap, int* __restrict__ count, DevOutputs out, int horizon) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+__device__ __forceinline__ void pack_ext2_one(const DevInputs& in, const uint32_t* __restrict__ sched, const double* __restrict__ normals, int b,
+                                              double* __restrict__ rec, int cap, int* __restrict__ count, const DevOutputs& out, int horizon) {
   unsigned long long s0 = 0ull, s1 = 0ull;
   bool two = true;
   for (int st = 0; st < horizon; ++st) {
@@ -149,14 +193,114 @@ __global__ void pack_ext2_kernel(DevInputs in, const uint32_t* __restrict__ sche
   }
 }
 
-// a1mpc_solve_batch_ext_warm: a robot without contact anywhere in its schedule never reaches a solve kernel (the pack kernels
-// answer it), so its warm-start slot is cleared here: it stores no guess, like a robot that ended NUMERICAL
-__global__ void warm_forget_no_contact_kernel(DevInputs in, const uint32_t* __restrict__ sched, int B, uint32_t* __restrict__ warm, int horizon) {
+__global__ void pack_ext2_kernel(DevInputs in, const uint32_t* __restrict__ sched, const double* __restrict__ normals, int B,
+                                 double* __restrict__ rec, int cap, int* __restrict__ count, DevOutputs out, int horizon) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
+  pack_ext2_one(in, sched, normals, b, rec, cap, count, out, horizon);
+}
+
+// a1mpc_solve_batch_ext_warm: a robot without contact anywhere in its schedule never reaches a solve kernel (the pack kernels
+// answer it), so its warm-start slot is cleared here: it stores no guess, like a robot that ended NUMERICAL
+__device__ __forceinline__ void warm_forget_one(const DevInputs& in, const uint32_t* __restrict__ sched, int b, uint32_t* __restrict__ warm, int horizon) {
   uint32_t any = 0u;
   for (int st = 0; st < horizon; ++st) any |= (sched ? sched[(size_t)st * in.ld + b] : in.contact[b]) & 15u;
   if (any == 0u) warm[(size_t)b * (WARM_HDR + 4 * horizon)] = 0u;
+}
+
+__global__ void warm_forget_no_contact_kernel(DevInputs in, const uint32_t* __restrict__ sched, int B, uint32_t* __restrict__ warm, int horizon) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  warm_forget_one(in, sched, b, warm, horizon);
+}
+
+// -------------------------------------------------------------------------------------------
+// the multi-rate tick (a1mpc_tick_set_mpc_period): robot b solves on its run n_b when n_b == 0 or n_b % period == b % period, and
+// the pack kernels below skip every other robot, so that it gets no record, no output store and no warm-slot write.  runs[b] is
+// n_b; tick_rate_kernel advances it after the solve.
+// -------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool mpc_due(uint32_t n, int b, int period) {
+  return n == 0u || n % (uint32_t)period == (uint32_t)b % (uint32_t)period;
+}
+
+__global__ void pack_due_kernel(DevInputs in, int B, double* __restrict__ rec, int cap, int* __restrict__ count, DevOutputs out, int horizon,
+                                const uint32_t* __restrict__ runs, int period) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B && mpc_due(runs[b], b, period)) pack_one(in, b, rec, cap, count, out, horizon);
+}
+
+__global__ void pack_ext_due_kernel(DevInputs in, const uint32_t* __restrict__ sched, const double* __restrict__ normals, int B,
+                                    double* __restrict__ rec, int* __restrict__ count, DevOutputs out, int horizon,
+                                    const uint32_t* __restrict__ runs, int period) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B && mpc_due(runs[b], b, period)) pack_ext_one(in, sched, normals, b, rec, count, out, horizon);
+}
+
+__global__ void pack_ext2_due_kernel(DevInputs in, const uint32_t* __restrict__ sched, const double* __restrict__ normals, int B,
+                                     double* __restrict__ rec, int cap, int* __restrict__ count, DevOutputs out, int horizon,
+                                     const uint32_t* __restrict__ runs, int period) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B && mpc_due(runs[b], b, period)) pack_ext2_one(in, sched, normals, b, rec, cap, count, out, horizon);
+}
+
+__global__ void warm_forget_no_contact_due_kernel(DevInputs in, const uint32_t* __restrict__ sched, int B, uint32_t* __restrict__ warm, int horizon,
+                                                  const uint32_t* __restrict__ runs, int period) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B && mpc_due(runs[b], b, period)) warm_forget_one(in, sched, b, warm, horizon);
+}
+
+// f_body = R^T u_full[12 step : 12 step + 12], the expression of the solve kernels' f_body = R^T u; a step at or past the horizon gives
+// zero forces.  rot [9][ld], u_full [12 N][ld], f_body [12][ld].
+__device__ __forceinline__ void plan_forces_one(int b, size_t ld, int horizon, const double* __restrict__ rot, const double* __restrict__ u_full,
+                                                uint32_t step, double* __restrict__ f_body) {
+  if (step >= (uint32_t)horizon) {
+#pragma unroll
+    for (int k = 0; k < 12; ++k) f_body[(size_t)k * ld + b] = 0.0;
+    return;
+  }
+  double R[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) R[k] = rot[(size_t)k * ld + b];
+  const double* u = u_full + (size_t)(12 * step) * ld + b;
+#pragma unroll
+  for (int leg = 0; leg < 4; ++leg) {
+    const double ux = u[(size_t)(3 * leg) * ld], uy = u[(size_t)(3 * leg + 1) * ld], uz = u[(size_t)(3 * leg + 2) * ld];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) f_body[(size_t)(3 * leg + a) * ld + b] = R[a] * ux + R[3 + a] * uy + R[6 + a] * uz;
+  }
+}
+
+// a1mpc_plan_forces_batch: step 0 leaves f_body alone (that run's solve wrote it)
+__global__ void plan_forces_kernel(int B, int horizon, const double* __restrict__ rot, const double* __restrict__ u_full,
+                                   const uint32_t* __restrict__ step, double* __restrict__ f_body) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const uint32_t s = step[b];
+  if (s != 0u) plan_forces_one(b, (size_t)B, horizon, rot, u_full, s, f_body);
+}
+
+// after the solve of a multi-rate tick: since[b] = j_b, the runs since robot b's last solve (0 on a solve run); with a plan (PLAYBACK_PLAN)
+// a robot that did not solve gets its plan's step j_b, rotated by this run's rot.  runs[b] = n_b + 1, taken back by `period` once it
+// reaches 2 period: that keeps n_b % period and n_b != 0, so the rule above never sees the counter wrap.
+__global__ void tick_rate_kernel(int B, int period, int horizon, uint32_t* __restrict__ runs, uint32_t* __restrict__ since,
+                                 const double* __restrict__ rot, const double* __restrict__ plan, double* __restrict__ f_body) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const uint32_t n = runs[b];
+  const bool due = mpc_due(n, b, period);
+  const uint32_t j = due ? 0u : since[b] + 1u;
+  since[b] = j;
+  if (plan && !due) plan_forces_one(b, (size_t)B, horizon, rot, plan, j, f_body);
+  const uint32_t next = n + 1u;
+  runs[b] = next >= 2u * (uint32_t)period ? next - (uint32_t)period : next;
+}
+
+// a1mpc_tick_reset_robots of a multi-rate tick: the masked robots solve on their next run
+__global__ void tick_rate_reset_kernel(int B, const uint8_t* __restrict__ mask, uint32_t* __restrict__ runs, uint32_t* __restrict__ since) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B || !mask[b]) return;
+  runs[b] = 0u;
+  since[b] = 0u;
 }
 
 // Classes whose factor does not fit in shared memory (N=20 with four stance feet in fp64):

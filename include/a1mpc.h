@@ -551,6 +551,31 @@ int  a1mpc_tick_set_terrain(a1mpc_tick* t, int source, const double* normals);
  * does not synchronise.  a1mpc_tick_reset and a1mpc_tick_reset_robots keep the source.  A1MPC_EINVAL: a NULL tick, an MPC-mode tick (it
  * takes a1mpc_tick_set_terrain), an unknown source, GIVEN with a NULL or host pointer. */
 int  a1mpc_tick_set_stance_terrain(a1mpc_tick* t, int source, const double* normals);
+/* Run an MPC-mode tick's solve at a lower rate than the tick.  The reference computes its ground forces in a thread of its own and the
+ * torque loop applies whatever forces that thread wrote last; here each robot solves on every period-th run, staggered across the batch,
+ * so that a run solves about B / period QPs instead of B.
+ *   Which robots solve: n_b counts robot b's runs since its start (create, a1mpc_tick_reset, its own a1mpc_tick_reset_robots or the
+ *   last a1mpc_tick_set_mpc_period).  Robot b solves on run n_b when n_b == 0 || n_b % period == b % period.  j_b, the runs since robot
+ *   b's last solve, stays in [0, period - 1].
+ *   On a robot's solve run, f_body and status come from the solve as on a plain tick.  On its other runs:
+ *     A1MPC_PLAYBACK_HOLD  f_body and status stay as its last solve wrote them (the reference's torque thread); nothing runs for it.
+ *     A1MPC_PLAYBACK_PLAN  f_body = R^T u_j with this run's R (rot) and u_j the world-frame forces of step j_b of its last solve's plan
+ *                          (u_full); status stays.  The plan advances one horizon step per run, which assumes that the handle's dt is the
+ *                          tick's period, as in the reference (mpc_dt = control period = 2.5 ms, a1mpc_default_config).
+ *   The torque stage uses this run's contacts either way: a force planned for a foot that has since lifted is not applied.
+ * The warm start keeps its shift on the held pattern (0, a guess `period` runs old is only a worse guess); the scheduled tick takes
+ * shift = period, as a due robot's stored faces are `period` schedule steps old.  A multi-rate tick does not take part in the fused
+ * collect.  period = 1 is the tick as if this call had never been made.  Every call makes every robot solve on its next run; the resets
+ * keep the period and the playback.  The first call with period > 1 allocates the tick's counters (and, for PLAN, its plan [12 N][B])
+ * and may synchronise; after it a run on device arrays still allocates nothing and does not synchronise.  A1MPC_EINVAL: a NULL tick,
+ * QP mode (the stance QP runs on every run), period outside [1, N] (N the handle's horizon), an unknown playback. */
+#define A1MPC_PLAYBACK_HOLD 0   /* between solves: f_body and status of the robot's last solve, unchanged */
+#define A1MPC_PLAYBACK_PLAN 1   /* between solves: R_now^T * u_j, step j of the last solve's world-frame plan */
+int  a1mpc_tick_set_mpc_period(a1mpc_tick* t, int period, int playback);
+/* The playback of A1MPC_PLAYBACK_PLAN as a staged entry point: rot [9][B], u_full [12 N][B] (as a1mpc_outputs.u_full), step [B] in,
+ * f_body [12][B] in/out, host or device.  step_b = 0 leaves robot b's f_body untouched (that run's solve wrote it); 1 <= step_b < N writes
+ * f_body = R^T u_full[12 step_b : 12 step_b + 12]; step_b >= N writes zero forces.  A1MPC_EINVAL: NULL handle or array, B <= 0. */
+int  a1mpc_plan_forces_batch(a1mpc_handle* h, int B, const double* rot, const double* u_full, const uint32_t* step, double* f_body);
 int  a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out);
 int  a1mpc_tick_destroy(a1mpc_tick* t);
 
