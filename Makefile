@@ -18,7 +18,7 @@ all: $(LIB) oracle host
 $(OBJ):
 	mkdir -p $(OBJ)
 
-$(OBJ)/%.o: $(SRC)/%.cu $(SRC)/a1mpc_device.cuh $(SRC)/a1mpc_hweig.h $(SRC)/a1mpc_sched.cuh $(SRC)/a1mpc_estim.cuh $(SRC)/a1mpc_swing.cuh $(SRC)/a1mpc_tick.cuh $(SRC)/a1mpc_filter.cuh $(SRC)/a1mpc_command.cuh $(SRC)/a1mpc_command_state.cuh $(SRC)/a1mpc_misc.cuh $(SRC)/a1mpc_solve_body.inc $(SRC)/a1mpc_sched_body.inc $(SRC)/a1mpc_solve_n10.cu $(SRC)/a1mpc_internal.h include/a1mpc.h | $(OBJ)
+$(OBJ)/%.o: $(SRC)/%.cu $(SRC)/a1mpc_device.cuh $(SRC)/a1mpc_hweig.h $(SRC)/a1mpc_sched.cuh $(SRC)/a1mpc_estim.cuh $(SRC)/a1mpc_swing.cuh $(SRC)/a1mpc_tick.cuh $(SRC)/a1mpc_filter.cuh $(SRC)/a1mpc_command.cuh $(SRC)/a1mpc_command_state.cuh $(SRC)/a1mpc_misc.cuh $(SRC)/a1mpc_gait.cuh $(SRC)/a1mpc_solve_body.inc $(SRC)/a1mpc_sched_body.inc $(SRC)/a1mpc_solve_n10.cu $(SRC)/a1mpc_internal.h include/a1mpc.h | $(OBJ)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $(OBJ)/$*.ptxas.log || (cat $(OBJ)/$*.ptxas.log; false)
 
 # the orientation / command stages round every product and sum as the reference does (no contraction into FMA)
@@ -36,6 +36,7 @@ oracle:
 	$(MAKE) -C oracle -s -f command.mk all ref
 	$(MAKE) -C oracle -s -f ekf_batch.mk all
 	$(MAKE) -C oracle -s -f stance_terrain.mk all
+	$(MAKE) -C oracle -s -f gait.mk ref
 
 host: $(LIB)
 	@if [ -f $(PKG)/host/Makefile ]; then $(MAKE) -C $(PKG)/host -s; fi

@@ -22,7 +22,7 @@ EXPORTS = [
     "a1mpc_grf_qp_batch", "a1mpc_stance_qp_batch", "a1mpc_stance_qp_batch_ext", "a1mpc_joint_torques_batch", "a1mpc_leg_kinematics_batch", "a1mpc_ekf_bytes", "a1mpc_ekf_init_batch", "a1mpc_ekf_update_batch", "a1mpc_update_plan_batch",
     "a1mpc_swing_bytes", "a1mpc_swing_init_batch", "a1mpc_swing_legs_batch", "a1mpc_terrain_pitch_batch", "a1mpc_terrain_normals_batch", "a1mpc_surface_normals_batch",
     "a1mpc_imu_bytes", "a1mpc_imu_init_batch", "a1mpc_orientation_batch", "a1mpc_command_bytes", "a1mpc_command_init_batch", "a1mpc_command_batch",
-    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_set_terrain", "a1mpc_tick_set_stance_terrain", "a1mpc_tick_set_mpc_period", "a1mpc_plan_forces_batch", "a1mpc_tick_run", "a1mpc_tick_destroy",
+    "a1mpc_default_tick_params", "a1mpc_tick_create", "a1mpc_tick_reset", "a1mpc_tick_reset_robots", "a1mpc_tick_set_terrain", "a1mpc_tick_set_stance_terrain", "a1mpc_tick_set_mpc_period", "a1mpc_tick_set_gaits", "a1mpc_gait_row", "a1mpc_update_plan_gait_batch", "a1mpc_swing_legs_gait_batch", "a1mpc_plan_forces_batch", "a1mpc_tick_run", "a1mpc_tick_destroy",
     "a1mpc_device_alloc", "a1mpc_device_free", "a1mpc_host_alloc", "a1mpc_host_free",
     "a1mpc_memcpy_h2d", "a1mpc_memcpy_d2h", "a1mpc_sync", "a1mpc_event_create", "a1mpc_event_destroy",
     "a1mpc_event_record", "a1mpc_event_elapsed_ms", "a1mpc_launch_count", "a1mpc_measure_fp64_peak",
@@ -82,6 +82,7 @@ def default_command_params(variant=VARIANT_GAZEBO):
 TICK_QP, TICK_MPC = 0, 1
 TERRAIN_FLAT, TERRAIN_ESTIMATED, TERRAIN_GIVEN = 0, 1, 2   # a1mpc_tick_set_terrain
 PLAYBACK_HOLD, PLAYBACK_PLAN = 0, 1                        # a1mpc_tick_set_mpc_period
+GAIT_TROT, GAIT_PACE, GAIT_BOUND, GAIT_PRONK, GAIT_WALK = 1, 2, 3, 4, 5   # a1mpc_gait_row
 
 
 class TickParams(C.Structure):
@@ -197,6 +198,11 @@ def lib():
         l.a1mpc_tick_set_terrain.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         l.a1mpc_tick_set_stance_terrain.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         l.a1mpc_tick_set_mpc_period.argtypes = [C.c_void_p, C.c_int, C.c_int]
+        l.a1mpc_tick_set_gaits.argtypes = [C.c_void_p, C.c_void_p]
+        l.a1mpc_gait_row.argtypes = [C.c_int, C.c_void_p]
+        l.a1mpc_update_plan_gait_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams)] + [C.c_void_p] * 14
+        l.a1mpc_swing_legs_gait_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(GaitParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_double] + [C.c_void_p] * 10
         l.a1mpc_plan_forces_batch.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 4
         l.a1mpc_tick_run.argtypes = [C.c_void_p, C.c_double, C.POINTER(TickInputs), C.POINTER(TickOutputs)]
         l.a1mpc_tick_destroy.argtypes = [C.c_void_p]
@@ -289,6 +295,14 @@ class DeviceBatch:
                 setattr(self, name, None)
 
 
+def gait_row(gait_type):
+    """a1mpc_gait_row: one robot's gait row [6] (offsets FL FR RL RR, counter_per_gait, counter_per_swing) of GAIT_TROT / _PACE / _BOUND /
+    _PRONK / _WALK; np.repeat(gait_row(t)[:, None], B, axis=1) makes the [6][B] rows of Tick.set_gaits"""
+    row = np.zeros(6)
+    _check(lib().a1mpc_gait_row(int(gait_type), _p(row)))
+    return row
+
+
 class Tick:
     """a whole control tick for B robots (a1mpc_tick_*): owns the controller state; raw sensor arrays in, joint torques out.
 
@@ -367,6 +381,22 @@ class Tick:
         on its other runs PLAYBACK_PLAN applies the step of its last solve's plan that belongs to the run, rotated by this run's rot, and
         PLAYBACK_HOLD keeps the forces and status of its last solve.  Every robot solves on the next run"""
         _check(lib().a1mpc_tick_set_mpc_period(self.t, int(period), int(playback)))
+
+    def set_gaits(self, rows):
+        """a1mpc_tick_set_gaits on host rows: float64 [6][B] (rows 0-3 the standstill counters FL FR RL RR, row 4 counter_per_gait, row 5
+        counter_per_swing; gait_row builds one column), or None for the reference's trot.  The rows are checked (a bad one raises A1MpcError
+        naming the robot and leaves the previous gaits in force); cps and cpg apply from the next run, the offsets when a robot stands"""
+        if rows is None:
+            self.set_gaits_ptr(0)
+            return
+        g = np.ascontiguousarray(rows, dtype=np.float64)
+        if g.shape != (6, self.B):
+            raise ValueError("gait rows must have shape (6, %d)" % self.B)
+        self.set_gaits_ptr(g.ctypes.data)
+
+    def set_gaits_ptr(self, ptr):
+        """a1mpc_tick_set_gaits on a pointer to [6][B] float64, e.g. a torch device tensor's data_ptr(); 0 returns to the trot"""
+        _check(lib().a1mpc_tick_set_gaits(self.t, ptr or None))
 
     def close(self):
         """a1mpc_tick_destroy; a tick whose Engine is closed has already been destroyed by Engine.close"""
@@ -705,6 +735,35 @@ class Engine:
         _check(lib().a1mpc_update_plan_batch(self.h, B, C.byref(gp), _p(gc), _p(a[0]), _p(mode), _p(a[1]), _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]),
                                              _p(plan), _p(sched), _p(trel), _p(tabs), _p(tw)))
         return gc, plan, sched, trel, tabs, tw
+
+    def update_plan_gait(self, gp, gait, gait_counter, gait_counter_speed, movement_mode, lin_vel, lin_vel_d, rot_z, rot, root_pos):
+        """a1mpc_update_plan_gait_batch: update_plan with each robot's gait row, gait [6,B]; returns what update_plan returns"""
+        g = np.ascontiguousarray(gait, dtype=np.float64)
+        gc = np.ascontiguousarray(gait_counter, dtype=np.float64).copy()
+        B = gc.shape[1]
+        if g.shape != (6, B):
+            raise ValueError("gait rows must have shape (6, %d)" % B)
+        a = [np.ascontiguousarray(v, dtype=np.float64) for v in (gait_counter_speed, lin_vel, lin_vel_d, rot_z, rot, root_pos)]
+        mode = np.ascontiguousarray(movement_mode, dtype=np.uint32)
+        plan = np.zeros(B, dtype=np.uint32); sched = np.zeros((gp.horizon, B), dtype=np.uint32)
+        trel = np.zeros((12, B)); tabs = np.zeros((12, B)); tw = np.zeros((12, B))
+        _check(lib().a1mpc_update_plan_gait_batch(self.h, B, C.byref(gp), _p(g), _p(gc), _p(a[0]), _p(mode), _p(a[1]), _p(a[2]), _p(a[3]), _p(a[4]),
+                                                  _p(a[5]), _p(plan), _p(sched), _p(trel), _p(tabs), _p(tw)))
+        return gc, plan, sched, trel, tabs, tw
+
+    def swing_legs_gait(self, gp, gait, kp_foot, kd_foot, swing, dt, gait_counter, plan_contacts, rot_z, foot_pos_abs, foot_pos_target_rel, foot_force):
+        """a1mpc_swing_legs_gait_batch: swing_legs with each robot's gait row, gait [6,B]; returns what swing_legs returns"""
+        g = np.ascontiguousarray(gait, dtype=np.float64)
+        kp, kd, gc = [np.ascontiguousarray(v, dtype=np.float64) for v in (kp_foot, kd_foot, gait_counter)]
+        pc = np.ascontiguousarray(plan_contacts, dtype=np.uint32)
+        a = [np.ascontiguousarray(v, dtype=np.float64) for v in (rot_z, foot_pos_abs, foot_pos_target_rel, foot_force)]
+        B = pc.shape[0]
+        if g.shape != (6, B):
+            raise ValueError("gait rows must have shape (6, %d)" % B)
+        fk = np.zeros((12, B)); con = np.zeros(B, dtype=np.uint32); cur = np.zeros((12, B)); rc = np.zeros((12, B))
+        _check(lib().a1mpc_swing_legs_gait_batch(self.h, B, C.byref(gp), _p(g), _p(kp), _p(kd), swing, C.c_double(dt), _p(gc), _p(pc),
+                                                 *[_p(v) for v in a], _p(fk), _p(con), _p(cur), _p(rc)))
+        return fk, con, cur, rc
 
     # ---- memory / timing helpers ----
     def dalloc(self, nbytes):

@@ -14,6 +14,7 @@
 #include "a1mpc_estim.cuh"
 #include "a1mpc_swing.cuh"
 #include "a1mpc_tick.cuh"
+#include "a1mpc_gait.cuh"
 
 using namespace a1mpc;
 
@@ -756,6 +757,49 @@ int a1mpc_update_plan_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp,
   return st.finish();
 }
 
+int a1mpc_gait_row(int gait_type, double row[6]) {
+  if (!row) return fail(A1MPC_EINVAL, "null argument");
+  // offsets FL FR RL RR, counter_per_gait, counter_per_swing; the trot is A1CtrlStates.h:24-25, 322-326
+  static const double rows[5][6] = {{0, 120, 120, 0, 240, 120},    // trot: diagonal pairs
+                                    {0, 120, 0, 120, 240, 120},    // pace: lateral pairs
+                                    {0, 0, 120, 120, 240, 120},    // bound: front pair, rear pair
+                                    {0, 0, 0, 0, 240, 120},        // pronk: all four
+                                    {120, 0, 180, 60, 240, 180}};  // lateral-sequence walk RL, FL, RR, FR, one foot in swing at a time
+  if (gait_type < A1MPC_GAIT_TROT || gait_type > A1MPC_GAIT_WALK) return fail(A1MPC_EINVAL, "unknown gait type");
+  for (int k = 0; k < 6; ++k) row[k] = rows[gait_type - A1MPC_GAIT_TROT][k];
+  return A1MPC_OK;
+}
+
+int a1mpc_update_plan_gait_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, const double* gait, double* gait_counter,
+                                 const double* gait_counter_speed, const uint32_t* movement_mode, const double* lin_vel, const double* lin_vel_d,
+                                 const double* rot_z, const double* rot, const double* root_pos, uint32_t* plan_contacts, uint32_t* contact_sched,
+                                 double* t_rel, double* t_abs, double* t_world) {
+  if (!h || !gp || !gait || !gait_counter || !gait_counter_speed || !movement_mode || !plan_contacts) return fail(A1MPC_EINVAL, "null argument");
+  const bool want_t = t_rel || t_abs || t_world;
+  if (want_t && (!lin_vel || !lin_vel_d || !rot_z || !rot || !root_pos)) return fail(A1MPC_EINVAL, "foothold targets need lin_vel, lin_vel_d, rot_z, rot, root_pos");
+  if (B <= 0 || gp->horizon < 0 || gp->horizon > A1MPC_MAX_HORIZON) return fail(A1MPC_EINVAL, "bad B or horizon");
+  CK(cudaSetDevice(h->device));
+  GaitDev G;
+  G.cpg = gp->counter_per_gait; G.cps = gp->counter_per_swing; G.cdt = gp->control_dt; G.dxl = gp->foot_delta_x_limit; G.dyl = gp->foot_delta_y_limit;
+  for (int i = 0; i < 12; ++i) G.dfp[i] = gp->default_foot_pos[i];
+  G.N = gp->horizon;
+  Stage st(h, B);
+  st.in(gait, 6); st.inout(gait_counter, 4); st.in(gait_counter_speed, 4); st.in(movement_mode, 1);
+  if (want_t) {
+    st.in(lin_vel, 3); st.in(lin_vel_d, 3); st.in(rot_z, 9); st.in(rot, 9); st.in(root_pos, 3);
+  } else {
+    for (const void* p : {lin_vel, lin_vel_d, rot_z, rot, root_pos}) st.unused(p);
+  }
+  st.out(plan_contacts, 1); st.out(contact_sched, G.N); st.out(t_rel, 12); st.out(t_abs, 12); st.out(t_world, 12);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  update_plan_gait_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, G, gait, gait_counter, gait_counter_speed, movement_mode, lin_vel, lin_vel_d,
+                                                                   rot_z, rot, root_pos, plan_contacts, contact_sched, t_rel, t_abs, t_world);
+  h->launches++;
+  CK(cudaGetLastError());
+  return st.finish();
+}
+
 // ---- upstream producers of the path's inputs (SURVEY 8f.4) ---------------------------------------------------
 
 int a1mpc_leg_kinematics_batch(a1mpc_handle* h, int B, const double* joint_pos, const double* joint_vel, const double* rot,
@@ -857,6 +901,36 @@ int a1mpc_swing_legs_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, 
   for (int i = 0; i < 12; ++i) { P.kp[i] = kp_foot[i]; P.kd[i] = kd_foot[i]; }
   swing_legs_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, P, static_cast<double*>(swing_state), gait_counter, plan_contacts, rot_z, foot_pos_abs,
                                                             foot_pos_target_rel, foot_force, f_kin, contacts, foot_pos_cur, foot_pos_recent_contact);
+  h->launches++;
+  CK(cudaGetLastError());
+  return st.finish();
+}
+
+int a1mpc_swing_legs_gait_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, const double* gait, const double* kp_foot, const double* kd_foot,
+                                void* swing_state, double dt, const double* gait_counter, const uint32_t* plan_contacts, const double* rot_z,
+                                const double* foot_pos_abs, const double* foot_pos_target_rel, const double* foot_force, double* f_kin, uint32_t* contacts,
+                                double* foot_pos_cur, double* foot_pos_recent_contact) {
+  if (!h || !gp || !gait || !kp_foot || !kd_foot || !swing_state || !gait_counter || !plan_contacts || !rot_z || !foot_pos_abs || !foot_pos_target_rel ||
+      !foot_force || !f_kin || !contacts)
+    return fail(A1MPC_EINVAL, "null argument");
+  if (B <= 0) return fail(A1MPC_EINVAL, "B must be positive");
+  if (!(dt > 0.0)) return fail(A1MPC_EINVAL, "dt must be positive");
+  CK(cudaSetDevice(h->device));
+  if (!is_device_ptr(swing_state)) return fail(A1MPC_EINVAL, "swing_state must be device memory (a1mpc_device_alloc)");
+  Stage st(h, B);
+  st.in(gait, 6); st.in(gait_counter, 4); st.in(plan_contacts, 1); st.in(rot_z, 9); st.in(foot_pos_abs, 12); st.in(foot_pos_target_rel, 12);
+  st.in(foot_force, 4);
+  st.out(f_kin, 12); st.out(contacts, 1); st.out(foot_pos_cur, 12); st.out(foot_pos_recent_contact, 12);
+  st.host_param(kp_foot, "kp_foot"); st.host_param(kd_foot, "kd_foot");
+  int rc;
+  if ((rc = st.begin())) return rc;
+  SwingParams P;
+  P.cps = gp->counter_per_swing;   // not read: each robot's row gives its own
+  P.dt = dt;
+  for (int i = 0; i < 12; ++i) { P.kp[i] = kp_foot[i]; P.kd[i] = kd_foot[i]; }
+  swing_legs_gait_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, P, gait, static_cast<double*>(swing_state), gait_counter, plan_contacts, rot_z,
+                                                                 foot_pos_abs, foot_pos_target_rel, foot_force, f_kin, contacts, foot_pos_cur,
+                                                                 foot_pos_recent_contact);
   h->launches++;
   CK(cudaGetLastError());
   return st.finish();
@@ -1047,6 +1121,11 @@ struct a1mpc_tick {
   void* rmem = nullptr;            // runs [B] (n_b), then since [B] (j_b)
   uint32_t *runs = nullptr, *since = nullptr;
   double* plan = nullptr;          // [12 N][B] each robot's u_full of its last solve (A1MPC_PLAYBACK_PLAN)
+  // per-robot gaits (a1mpc_tick_set_gaits); gmem is allocated by the first call with rows
+  void* gmem = nullptr;            // gait [6][B], then the row check's result word
+  double* gait = nullptr;
+  unsigned long long* gbad = nullptr;
+  bool gaits = false;              // the front runs its gait twin on `gait`
 };
 
 namespace {
@@ -1343,6 +1422,51 @@ int a1mpc_tick_set_mpc_period(a1mpc_tick* t, int period, int playback) {
   return A1MPC_OK;
 }
 
+int a1mpc_tick_set_gaits(a1mpc_tick* t, const double* gait) {
+  if (!t) return fail(A1MPC_EINVAL, "null argument");
+  if (!gait) {   // the reference's trot: tp.gait and the trot offsets
+    t->gaits = false;
+    return A1MPC_OK;
+  }
+  a1mpc_handle* h = t->h;
+  const int B = t->B;
+  const size_t lb = (size_t)B;
+  CK(cudaSetDevice(h->device));
+  const size_t rows_bytes = (6 * lb * sizeof(double) + 255) & ~(size_t)255;
+  if (!t->gmem) {
+    if (cudaMalloc(&t->gmem, rows_bytes + sizeof(unsigned long long)) != cudaSuccess) {
+      cudaGetLastError();
+      t->gmem = nullptr;
+      return fail(A1MPC_ENOMEM, "cudaMalloc failed");
+    }
+    t->gait = static_cast<double*>(t->gmem);
+    t->gbad = reinterpret_cast<unsigned long long*>(static_cast<char*>(t->gmem) + rows_bytes);
+  }
+  // the rows are checked where they are (host rows in the staging slot) and copied into the tick only when every one is valid, so a
+  // bad call leaves the previous gaits in force
+  Stage st(h, B);
+  st.in(gait, 6);
+  int rc;
+  if ((rc = st.begin())) return rc;
+  CK(cudaMemsetAsync(t->gbad, 0xff, sizeof(unsigned long long), h->stream));
+  gait_check_kernel<<<(B + 127) / 128, 128, 0, h->stream>>>(B, gait, t->gbad);
+  h->launches++;
+  CK(cudaGetLastError());
+  unsigned long long bad = 0;
+  CK(cudaMemcpyAsync(&bad, t->gbad, sizeof(bad), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  if (bad != ~0ull) {
+    static const char* rule[4] = {"", "a non-finite entry", "counter_per_swing (row 5) outside (0, counter_per_gait)",
+                                  "a reset offset (rows 0-3) outside [0, counter_per_gait)"};
+    return fail(A1MPC_EINVAL, "gait row of robot " + std::to_string(bad >> 2) + ": " + rule[bad & 3ull]);
+  }
+  // the call returns with the rows in the tick: the caller may rewrite or free its array at once, from any stream
+  CK(cudaMemcpyAsync(t->gait, gait, 6 * lb * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  t->gaits = true;
+  return A1MPC_OK;
+}
+
 int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out) {
   if (!t || !in || !out || !out->tau) return fail(A1MPC_EINVAL, "null argument");
   if (!in->quat || !in->gyro || !in->acc || !in->joint_pos || !in->joint_vel || !in->foot_force || !in->cmd || !in->gait_counter_speed)
@@ -1385,7 +1509,13 @@ int a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const 
     SP.dt = dt;
     for (int i = 0; i < 12; ++i) { SP.kp[i] = tp.kp_foot[i]; SP.kd[i] = tp.kd_foot[i]; }
     const double* lvd = mpc ? t->ref + 5 * lb : t->des + 6 * lb;
-    if (t->sched)
+    if (t->gaits && t->sched)
+      tick_front_sched_gait<<<(B + 127) / 128, 128, 0, h->stream>>>(B, LP, G, SP, t->gait, jp, jv, t->rot, t->rz, t->x0, lvd, t->mode, t->gc, gcs,
+                                                                    t->swing, ff, t->fpr, t->jac, t->fvr, t->foot, t->fk, t->contact, t->sched);
+    else if (t->gaits)
+      tick_front_b_gait<<<(B + 127) / 128, 128, 0, h->stream>>>(B, LP, G, SP, t->gait, jp, jv, t->rot, t->rz, t->x0, lvd, t->mode, t->gc, gcs, t->swing,
+                                                                ff, t->fpr, t->jac, t->fvr, t->foot, t->fk, t->contact);
+    else if (t->sched)
       tick_front_sched<<<(B + 127) / 128, 128, 0, h->stream>>>(B, LP, G, SP, jp, jv, t->rot, t->rz, t->x0, lvd, t->mode, t->gc, gcs, t->swing, ff,
                                                                t->fpr, t->jac, t->fvr, t->foot, t->fk, t->contact, t->sched);
     else
@@ -1487,6 +1617,7 @@ int a1mpc_tick_destroy(a1mpc_tick* t) {
   if (t->mem) cudaFree(t->mem);
   if (t->tmem) cudaFree(t->tmem);
   if (t->rmem) cudaFree(t->rmem);
+  if (t->gmem) cudaFree(t->gmem);
   if (t->plan) cudaFree(t->plan);
   delete t;
   return A1MPC_OK;

@@ -324,6 +324,30 @@ int  a1mpc_update_plan_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp
                              const uint32_t* movement_mode, const double* lin_vel, const double* lin_vel_d, const double* rot_z,
                              const double* rot, const double* root_pos, uint32_t* plan_contacts, uint32_t* contact_sched,
                              double* foot_pos_target_rel, double* foot_pos_target_abs, double* foot_pos_target_world);
+/* Per-robot gaits.  A gait row is six numbers per robot, gait [6][B] batch-major (host or device, like the other arrays):
+ *   rows 0-3  the counters a standing robot is reset to, FL FR RL RR (the robot's own gait_counter_reset(), A1CtrlStates.h:322-326)
+ *   row 4     counter_per_gait (cpg)
+ *   row 5     counter_per_swing (cps: a leg is planned in contact while its counter is <= cps, so cps is the stance length)
+ * A valid row is finite, with 0 < cps < cpg and every offset in [0, cpg).  The swing lasts cpg - cps counts: the swing spline time is
+ * float(gc - cps) / float(cpg - cps) and the early-contact threshold the middle of the swing, cps + 0.5 (cpg - cps); the foothold's
+ * (cps / speed) * control_dt / 2 and the schedule's fmod(c + st * speed, cpg) <= cps take the robot's own cps and cpg.  With cpg = 2 cps
+ * (the default 240 / 120) every one of them is the reference's expression to the bit.
+ * a1mpc_gait_row fills one row: A1MPC_GAIT_TROT is the reference's gait_type 1, the only one it fills in.  At equal leg speeds the pace
+ * swings the lateral pairs together, the bound the front and the rear pair, the pronk all four feet (a flight phase with no foot down);
+ * the walk is a lateral-sequence walk (RL, FL, RR, FR a quarter cycle apart, cps = 3/4 cpg) with at most one foot in swing.
+ * A1MPC_EINVAL for an unknown type or a NULL row. */
+#define A1MPC_GAIT_TROT  1   /* offsets 0 120 120 0,   cpg 240, cps 120 */
+#define A1MPC_GAIT_PACE  2   /* offsets 0 120 0 120,   cpg 240, cps 120 */
+#define A1MPC_GAIT_BOUND 3   /* offsets 0 0 120 120,   cpg 240, cps 120 */
+#define A1MPC_GAIT_PRONK 4   /* offsets 0 0 0 0,       cpg 240, cps 120 */
+#define A1MPC_GAIT_WALK  5   /* offsets 120 0 180 60,  cpg 240, cps 180 */
+int  a1mpc_gait_row(int gait_type, double row[6]);
+/* a1mpc_update_plan_batch with each robot's gait row: gait [6][B] replaces gp's counter_per_gait and counter_per_swing and the trot
+ * reset; gp gives the rest.  The rows are not checked here (a1mpc_tick_set_gaits checks them). */
+int  a1mpc_update_plan_gait_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, const double* gait, double* gait_counter,
+                                  const double* gait_counter_speed, const uint32_t* movement_mode, const double* lin_vel, const double* lin_vel_d,
+                                  const double* rot_z, const double* rot, const double* root_pos, uint32_t* plan_contacts, uint32_t* contact_sched,
+                                  double* foot_pos_target_rel, double* foot_pos_target_abs, double* foot_pos_target_world);
 
 /* ---- the stages between update_plan and the path: A1RobotControl::generate_swing_legs_ctrl and compute_grf's terrain adaptation ----
  * generate_swing_legs_ctrl (A1RobotControl.cpp:204-287) produces the `contact` of a1mpc_solve_batch* and the f_kin / contact of
@@ -368,6 +392,12 @@ int  a1mpc_swing_legs_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp,
                             double dt, const double* gait_counter, const uint32_t* plan_contacts, const double* rot_z, const double* foot_pos_abs,
                             const double* foot_pos_target_rel, const double* foot_force, double* f_kin, uint32_t* contacts, double* foot_pos_cur,
                             double* foot_pos_recent_contact);
+/* a1mpc_swing_legs_batch with each robot's gait row gait [6][B] (a1mpc_update_plan_gait_batch): cps and cpg come from the row (gp's
+ * counter_per_swing is not read), with the spline time and early-contact threshold of the gait rows above. */
+int  a1mpc_swing_legs_gait_batch(a1mpc_handle* h, int B, const a1mpc_gait_params* gp, const double* gait, const double* kp_foot, const double* kd_foot,
+                                 void* swing_state, double dt, const double* gait_counter, const uint32_t* plan_contacts, const double* rot_z,
+                                 const double* foot_pos_abs, const double* foot_pos_target_rel, const double* foot_force, double* f_kin,
+                                 uint32_t* contacts, double* foot_pos_cur, double* foot_pos_recent_contact);
 int  a1mpc_terrain_pitch_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref, size_t ref_ld,
                                double* terrain_pitch);
 int  a1mpc_terrain_normals_batch(a1mpc_handle* h, int B, void* swing_state, int use_terrain_adapt, const double* root_pos, double* ref,
@@ -576,6 +606,21 @@ int  a1mpc_tick_set_mpc_period(a1mpc_tick* t, int period, int playback);
  * f_body [12][B] in/out, host or device.  step_b = 0 leaves robot b's f_body untouched (that run's solve wrote it); 1 <= step_b < N writes
  * f_body = R^T u_full[12 step_b : 12 step_b + 12]; step_b >= N writes zero forces.  A1MPC_EINVAL: NULL handle or array, B <= 0. */
 int  a1mpc_plan_forces_batch(a1mpc_handle* h, int B, const double* rot, const double* u_full, const uint32_t* step, double* f_body);
+/* Give each robot of a tick its own gait (both modes): gait [6][B], the rows of a1mpc_gait_row / a1mpc_update_plan_gait_batch, host or
+ * device.  The rows are checked on the device and copied into the tick; the call synchronises (twice: after the check, and after the
+ * copy, so that it returns with the rows in the tick and the caller may rewrite or free its array at once, from any stream).  A bad row gives A1MPC_EINVAL naming
+ * the first bad robot and the rule it breaks, and the previous gaits stay in force.  gait = NULL returns to the reference's trot (tp.gait's
+ * cpg and cps, offsets 0 120 120 0): a tick that never made this call, or made it with NULL, runs exactly as before.
+ *   cps and cpg apply from the next run.  The offsets apply when a robot stands, where the reference calls gait_counter_reset(): a walking
+ *   robot keeps its leg phases until it stops (no gait-transition planner).
+ *   a1mpc_tick_reset and a1mpc_tick_reset_robots keep the gaits.  A reset robot starts in standstill (joy_cmd_ctrl_state 0), so unless its
+ *   first run's cmd toggles walking it takes its row's offsets on that run.  To re-phase robots: set the gaits, then reset those robots; or,
+ *   without a reset, toggle them to standstill for one run with cmd row 6 and back to walking on a later run.
+ *   The first non-NULL call allocates 6 B doubles in the tick; after it a run on device arrays allocates nothing and does not synchronise.
+ *   A pronk's flight phase gives robots with no stance foot: they take the existing no-contact path (A1MPC_STATUS_NO_CONTACT, zero
+ *   forces) in both modes.
+ * A1MPC_EINVAL: a NULL tick, a bad row. */
+int  a1mpc_tick_set_gaits(a1mpc_tick* t, const double* gait);
 int  a1mpc_tick_run(a1mpc_tick* t, double dt, const a1mpc_tick_inputs* in, const a1mpc_tick_outputs* out);
 int  a1mpc_tick_destroy(a1mpc_tick* t);
 
